@@ -1,10 +1,10 @@
 #!/usr/bin/env python
-"""bench.py — stage-2 k-mers/s (k=31) of the B200 path on BASELINE.json's target workload, next to the reference's CPU stage 2.
+"""bench.py — stage-2 k-mers/s (k=31) of the H100 path on BASELINE.json's target workload, next to the reference's CPU stage 2.
 
 Workload (BASELINE configs[2], SURVEY 8d "config 3"): 512 bins of a 30x human-like run, ~6.1e10 k-mers in total, k=31 canonical,
 ci=2 cx=1e9 cs=255 p=7.  The 512 bins are drawn from a pool of 8 distinct synthetic bins (kb_collector format, ~12 k-mers per
-super-k-mer, 30x duplicate-rich, 1 % substitutions) whose sizes are spread Zipf-like over 2^25 .. 2^28 k-mers (mean 1.2e8, so the
-9-bit second partition level is the common case).  A "step" = all 512 bins once.  STRONG scaling: the bins are sharded over the
+super-k-mer, 30x duplicate-rich, 1 % substitutions) whose sizes are spread Zipf-like over 2^25 .. 2^28 k-mers (mean 1.2e8 k-mers per
+bin).  A "step" = all 512 bins once.  STRONG scaling: the bins are sharded over the
 ranks in the reference's order - descending size, each to the least-loaded rank (kmc_b200.sharding.assign_bins = LPT, what N sorter
 objects pulling from one CBinQueue in get_sorted_req_sizes order converge to; kmc_core/kmc.h:1564-1600, queues.h:499-558) - and no
 collective touches the data path.
@@ -20,7 +20,13 @@ collective touches the data path.
               host cores over a bounded, size-stratified sample of the SAME 512 bins; the warm-up steps sweep the reference's
               concurrency (arena size = bins in flight, sorter threads) and the timed steps use the best setting
 
-Usage: python bench.py [--gpus N] [--steps K] [--warmup W] [--impl ours|reference] [--scale S] [--no-cpu] [--no-secondary]
+  --dump-outputs DIR : after the timed steps, what the device-resident path handed back in its last step, as .npy (float64):
+              step_results (the 8 result words of every bin of the step, in processing order), and of the step's last bin
+              (the one whose records are still in the output buffer) lut, suffix (the suffix bytes of every emitted record as one
+              integer, < 2^53) and count; a fixed, seeded sample of the records when there are more than DUMP_MAX_RECORDS
+              (the inputs are seeded, so two builds run with the same arguments can be compared array by array)
+
+Usage: python bench.py [--gpus N] [--steps K] [--warmup W] [--impl ours|reference] [--scale S] [--no-cpu] [--no-secondary] [--dump-outputs DIR]
 """
 import argparse
 import json
@@ -50,6 +56,7 @@ POOL_MI = [256, 192, 160, 128, 112, 96, 64, 32]        # k-mers per pool bin, in
 POOL_COUNT = [24, 40, 56, 72, 96, 96, 80, 48]          # how often each occurs among the 512 bins (Zipf-like: few large, many small)
 N_BINS = sum(POOL_COUNT)
 GEN_CHUNK = 1 << 24
+DUMP_MAX_RECORDS = 1 << 21             # --dump-outputs: at most this many records of the last bin (suffix + count: 16 bytes each, 32 MiB)
 
 
 def hbm_peak():
@@ -59,7 +66,7 @@ def hbm_peak():
             return float(json.load(open(p))["hbm_gbs"]), "measured (MEASURED_PEAKS.json hbm_gbs)"
         except Exception:
             pass
-    return 6650.0, "fallback (B200_PROFILING.md)"
+    return 3350.0, "H100 SXM data sheet (HBM3, 3.35 TB/s)"
 
 
 # ------------------------------------------------------------------------------------------------ workload
@@ -112,13 +119,13 @@ def workload_config(scale, n_gpus, sizes):
         "bin_pool_kmers": sizes, "bin_pool_count": POOL_COUNT, "scale_divisor": scale,
         "bin": "synthetic super-k-mers (kb_collector format), ~12 k-mers/super-k-mer, 30x duplicate-rich, 1% substitutions",
         "sharding": "LPT over descending bin size (kmc_b200.sharding.assign_bins), %d rank(s), no collective on the data path" % n_gpus,
-        "l2": "every bin's working set (2 record buffers of 8 B x 3e7..2.7e8 records) >> 126 MB L2; consecutive bins differ",
+        "l2": "every bin's working set (2 record buffers of 8 B x 3e7..2.7e8 records) >> the H100's 50 MB L2; consecutive bins differ",
     }
 
 
 class ClockSampler:
     """nvidia-smi clocks/throttle reasons DURING the timed region."""
-    Q = "clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.hw_slowdown,clocks_event_reasons.hw_thermal_slowdown,clocks_event_reasons.sw_thermal_slowdown,clocks_event_reasons.sw_power_cap"
+    Q = "clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.hw_slowdown,clocks_event_reasons.hw_thermal_slowdown,clocks_event_reasons.sw_thermal_slowdown,clocks_event_reasons.sw_power_cap,power.limit"
 
     def __init__(self, index):
         self.index = index
@@ -146,7 +153,7 @@ class ClockSampler:
             self.proc.wait(timeout=2)
         except Exception:
             self.proc.kill()
-        sm, mx, reasons, pw = [], [], set(), []
+        sm, mx, reasons, pw, lim = [], [], set(), [], []
         names = ["hw_slowdown", "hw_thermal_slowdown", "sw_thermal_slowdown", "sw_power_cap"]
         for l in self.lines:
             f = [x.strip() for x in l.split(",")]
@@ -159,8 +166,12 @@ class ClockSampler:
             for n, v in zip(names, f[3:7]):
                 if v.lower().startswith("active"):
                     reasons.add(n)
+            try:
+                lim.append(float(f[7]))
+            except (IndexError, ValueError):
+                pass
         return {"sm_mhz": statistics.median(sm) if sm else None, "sm_min_mhz": min(sm) if sm else None, "sm_max_mhz": max(mx) if mx else None,
-                "power_w_max": max(pw) if pw else None, "power_w_median": statistics.median(pw) if pw else None,
+                "power_w_max": max(pw) if pw else None, "power_w_median": statistics.median(pw) if pw else None, "power_limit_w": max(lim) if lim else None,
                 "samples": len(sm), "reasons": sorted(reasons)}
 
 
@@ -267,7 +278,7 @@ def main_reference(args, rank, world):
             "config": workload_config(args.scale, args.gpus, sizes)}
     R = reference_lib()
     if R is None:
-        base["unavailable"] = "oracle/_ref/libkmc_ref.so was not built (needs /root/reference at build time)"
+        base["unavailable"] = "oracle/_ref/libkmc_ref.so was not built (build() compiles it from the KMC source tree that oracle/Makefile's REF or KMC_REFERENCE_DIR names)"
         print(json.dumps(base))
         return
     pool = make_pool(args.scale)
@@ -286,6 +297,25 @@ def main_reference(args, rank, world):
                  "e2e": {"value": value, "unit": UNIT, "h2d_bytes_per_step": 0, "d2h_bytes_per_step": 0},
                  "gpu_launches": 0})
     print(json.dumps(base))
+
+
+def dump_outputs(out_dir, res_rows, payload, lut, rec_bytes):
+    """The arrays of the last timed step (see --dump-outputs) as DIR/<name>.npy, float64: every value is an integer below 2^53."""
+    import numpy as np
+    os.makedirs(out_dir, exist_ok=True)
+    n = payload.size // rec_bytes
+    rec = payload[:n * rec_bytes].reshape(n, rec_bytes)
+    if n > DUMP_MAX_RECORDS:
+        rec = rec[np.sort(np.random.default_rng(2024).choice(n, DUMP_MAX_RECORDS, replace=False))]
+    suf_bytes = (K - LUT_P) // 4
+    suffix = np.zeros(rec.shape[0], dtype=np.uint64)
+    for j in range(suf_bytes):
+        suffix = (suffix << np.uint64(8)) | rec[:, j].astype(np.uint64)
+    count = np.zeros(rec.shape[0], dtype=np.uint64)
+    for j in range(rec_bytes - 1, suf_bytes - 1, -1):
+        count = (count << np.uint64(8)) | rec[:, j].astype(np.uint64)
+    for name, a in (("step_results", res_rows), ("last_bin_lut", lut), ("last_bin_suffix", suffix), ("last_bin_count", count)):
+        np.save(os.path.join(out_dir, name + ".npy"), np.asarray(a).astype(np.float64))
 
 
 # ------------------------------------------------------------------------------------------------ our arm
@@ -525,6 +555,11 @@ def main_ours(args, rank, world, local_rank):
     barrier()
     dev_ms = e0.elapsed_time(e1)
     launches = ctx.kernel_launches() - launches0
+    if args.dump_outputs and rank == 0 and args.steps > 0:
+        last = (args.steps - 1) * n_my
+        rows = d_res[last:last + len(my)].cpu().numpy()
+        nb = int(rows[-1][4]) * ctx.out_rec_bytes if len(my) else 0
+        dump_outputs(args.dump_outputs, rows, d_out[:nb].cpu().numpy(), d_lut.cpu().numpy().view(np.uint64), ctx.out_rec_bytes)
     # every bin of every timed step is checked (not only the warm-up): statistics, emitted records, no error / fallback flag
     res_all = d_res.cpu().numpy()
     fallbacks = 0
@@ -601,28 +636,18 @@ def main_ours(args, rank, world, local_rank):
         gbs = lambda nm: alg[nm] / (acc[nm] * 1e-3) / 1e9 if acc.get(nm, 0) > 0 else None
         kernel_names = {"expand": "walk_packs_parallel_kernel + scan_packs_kernel + tile_desc_kernel + expand_kernel<1> (index + expansion of a bin)",
                         "msd_partition_L1": "msd_partition_kernel<1> (level-1 8-bit MSD partition pass)",
-                        "msd_partition_L2": "msd_partition_kernel<1,256|1024> (level-2 MSD partition pass, 8-9 bits)",
+                        "msd_partition_L2": "msd_partition_kernel<1> (level-2 MSD partition pass, 8 bits)",
                         "msd_count_L2": "msd_count_kernel<1> + cell scan (level-2 digit counts)",
                         "leaf_count": "leaf_hash_kernel<10> + leaf_scan/gather (count the leaves, emit the database records)"}
-        traffic, traffic_src = None, None
-        tp = os.path.join(ROOT, "profiles", "dominant_kernel_traffic.json")
-        if os.path.exists(tp):
-            try:
-                tj = json.load(open(tp))
-                if dom in tj.get("stages", {}):
-                    traffic = tj["stages"][dom]["dram_bytes_per_launch"]
-                    traffic_src = "%s; kernel %s" % (tj.get("source"), tj["stages"][dom].get("kernel"))
-            except Exception:
-                pass
         n_w = sum(weights)
         passes = {nm: {"ms_per_mean_bin": acc[nm] / n_w, "algorithmic_bytes_per_mean_bin": alg[nm] / n_w, "GB/s": gbs(nm), "frac": gbs(nm) / peak}
                   for nm in acc if nm.startswith("msd_partition") and acc[nm] > 0}
         out = {
-            "metric": METRIC, "value": value, "unit": UNIT, "n_gpus": world, "steps": args.steps, "warmup": args.warmup,
+            "metric": METRIC, "value": value, "unit": UNIT, "n_gpus": world, "gpu": torch.cuda.get_device_name(dev), "steps": args.steps, "warmup": args.warmup,
             "ms_per_step": dev_ms / args.steps, "higher_is_better": True, "scaling": "strong", "vs_baseline": None,
             "dtype": "u64", "data": "synthetic", "config": workload_config(args.scale, world, sizes),
             "roofline": {"bound": "hbm", "kernel": kernel_names.get(dom, dom), "stage": dom, "share_of_step": share[dom],
-                         "achieved": gbs(dom), "peak": peak, "unit": "GB/s", "frac": gbs(dom) / peak, "traffic": traffic, "traffic_source": traffic_src,
+                         "achieved": gbs(dom), "peak": peak, "unit": "GB/s", "frac": gbs(dom) / peak,
                          "peak_source": peak_src, "algorithmic_bytes_per_launch": alg[dom] / n_w, "avg_launch_ms": acc[dom] / n_w,
                          "how": "CUDA events recorded by the library around every stage of each of the 8 pool bins (after the timed region), weighted by how often the bin occurs among the 512",
                          "passes": passes,
@@ -664,6 +689,7 @@ def main():
     ap.add_argument("--scale", type=int, default=int(os.environ.get("KMCB200_BENCH_SCALE", "1")), help="divide every bin size by this (development runs)")
     ap.add_argument("--no-cpu", action="store_true", help="skip the cpu_baseline leg (profiling runs)")
     ap.add_argument("--no-secondary", action="store_true", help="skip the secondary workloads (profiling runs)")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None, help="write what the timed path computed in its last step to DIR/<name>.npy")
     args = ap.parse_args()
     args.warmup = max(args.warmup, 3) if args.impl == "ours" else args.warmup
     rank = int(os.environ.get("RANK", "0"))

@@ -1,4 +1,4 @@
-/* kmc_b200 — C ABI of the B200 (sm_100a) implementation of KMC's per-bin stage 2.
+/* kmc_b200 — C ABI of the H100 (sm_90a) implementation of KMC's per-bin stage 2.
  *
  * This is the drop-in boundary: a KMC build binds these entry points where its own CPU code does the
  * per-bin work today.  File:line references are to refresh-bio/KMC 3.2.4.
@@ -16,7 +16,7 @@
  * Conventions: plain C types only; every function returns 0 on success or a negative kmcb200_status;
  * kmcb200_last_error() gives the message.  A context is bound to one GPU and may be used by one host
  * thread at a time (KMC runs one sorter thread per context).  There is NO CPU fallback: without a usable
- * sm_100 device kmcb200_create fails with KMCB200_ERR_NO_DEVICE.
+ * sm_90 device kmcb200_create fails with KMCB200_ERR_NO_DEVICE.
  *
  * Environment knobs read by kmcb200_create (development / tests; the defaults are the measured best):
  *   KMCB200_SORT=lsd               plain 8-bit LSD passes instead of the hybrid MSD sort
@@ -25,8 +25,8 @@
  *   KMCB200_LEAF_KERNEL=warp       round 1's leaf kernel (ordered groups, leaf_warp.cuh) instead of leaf_hash_kernel; KMCB200_LEAF_WIDE=warp: for records of > 1 word only
  *   KMCB200_LEAF_FILL_PCT=n        leaf_hash_kernel plans a table round for this load (default 62); KMCB200_LEAF_RATIO0=n: first guess of distinct k-mers per record x 256 (default 90)
  *   KMCB200_LEAF_ROUND_PCT=n       leaf_warp_kernel: records per table round in percent of the slots (default 100)
- *   KMCB200_L2_BITS=1..10          bits of the second partition level (default: from the bin size: 8, from ~10^8 one-word k-mers on 9; wider records up to 10)
- *   KMCB200_LEAF_TARGET=n, KMCB200_LEAF_MAX_B2=8..10   mean leaf size / most bits the default rule aims at for one-word records (1024, 9)
+ *   KMCB200_L2_BITS=1..10          bits of the second partition level (default: from the bin size: 8 for one-word records; wider records up to 10)
+ *   KMCB200_LEAF_TARGET=n, KMCB200_LEAF_MAX_B2=8..10   mean leaf size / most bits the default rule aims at for one-word records (1024, 8)
  *   KMCB200_MAX_BLOCK_RECORDS=n    a bin with more k-mers is counted key block by key block (default: what 60 % of the free HBM holds, < 2^32)
  *   KMCB200_KEY_BLOCKS=filter     key blocks of an oversized bin re-expand it with a filter (default: one scattering expansion when the records fit in HBM once)
  *   KMCB200_KEY_BLOCK_RECORDS=n    preferred size of a key block in the scattering flow (default 2^28)
@@ -50,7 +50,7 @@ extern "C" {
 typedef enum {
 	KMCB200_OK = 0,
 	KMCB200_ERR_INVALID = -1,             /* bad argument */
-	KMCB200_ERR_NO_DEVICE = -2,           /* no CUDA device / not sm_100 */
+	KMCB200_ERR_NO_DEVICE = -2,           /* no CUDA device / not sm_90 (H100) */
 	KMCB200_ERR_CUDA = -3,                /* CUDA runtime error (message in last_error) */
 	KMCB200_ERR_BIN_FORMAT = -4,          /* packs do not end on record boundaries / n_rec mismatch */
 	KMCB200_ERR_CAPACITY = -5,            /* out_capacity too small */

@@ -1,9 +1,9 @@
-"""kmc_b200 — Python host side over the C ABI (include/kmc_b200.h) of the B200 stage-2 path of KMC.
+"""kmc_b200 — Python host side over the C ABI (include/kmc_b200.h) of the H100 stage-2 path of KMC.
 
 The product is the CUDA library `libkmc_b200.so` (kmc_b200/csrc); this module is a thin ctypes mirror used
 by the tests and by bench.py.  Names follow the reference: a *bin* of super-k-mers goes through
 Expand -> Sort -> Compact exactly like `CKmerBinSorter<SIZE>::ProcessBins` (kmc_core/kb_sorter.h:210-237).
-There is no CPU fallback: constructing a `Stage2Context` without a B200 raises.
+There is no CPU fallback: constructing a `Stage2Context` without an H100 raises.
 """
 import ctypes as C
 import os

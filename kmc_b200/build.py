@@ -1,4 +1,4 @@
-"""Builds kmc_b200/libkmc_b200.so in-tree with nvcc for sm_100a (no JIT cache: the .so travels with the repo)."""
+"""Builds kmc_b200/libkmc_b200.so in-tree with nvcc for sm_90a (H100; no JIT cache: the .so is built once, next to the package)."""
 import os
 import subprocess
 import sys
@@ -9,7 +9,7 @@ DEPS = sorted(os.path.join(HERE, "csrc", f) for f in os.listdir(os.path.join(HER
     os.path.join(os.path.dirname(HERE), "include", "kmc_b200.h")]
 OUT = os.path.join(HERE, "libkmc_b200.so")
 NVCC = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
-FLAGS = ["-gencode", "arch=compute_100a,code=sm_100a", "-lineinfo", "-O3", "-std=c++17", "--shared", "-Xcompiler", "-fPIC",
+FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-O3", "-std=c++17", "--shared", "-Xcompiler", "-fPIC",
          "-Xcompiler", "-fvisibility=default"]
 
 

@@ -1,4 +1,4 @@
-// kmc_b200 — device-side helpers shared by the stage-2 kernels (sm_100a only).
+// kmc_b200 — device-side helpers shared by the stage-2 kernels (sm_90a only).
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>

@@ -95,7 +95,7 @@ __device__ __forceinline__ uint64_t tile_first_base(uint64_t pack_start, uint32_
 // The rest is repaired, not assumed: the entry of segment t must be exactly the exit of segment t-1 (segment 0 starts on the
 // true start); a segment whose entry is off re-walks from the true one, round after round until nothing changes (chains merge,
 // so exits rarely move: one or two rounds).  A final check of the whole chain guards the result; a pack that fails it is left
-// to the exact warp-per-pack walker below.  A step costs one shared-memory load (~45 cycles); ~150 steps per thread.
+// to the exact warp-per-pack walker below.  A step costs one shared-memory load; ~150 steps per thread.
 constexpr int kWalkSegBytes = 256;
 constexpr int kWalkSegs = 256;                                   // threads per CTA = segments per pack
 constexpr int kWalkChunk = kWalkSegBytes * kWalkSegs;            // 64 KiB
@@ -200,7 +200,7 @@ __global__ void __launch_bounds__(kWalkSegs, 3) walk_packs_parallel_kernel(const
 // One WARP per pack.  The walk itself is a serial chain (the length byte of a record tells where the next one
 // starts), so the only thing that matters is the latency of one step.  The warp keeps a 512-byte window of the stream
 // in registers (one uint4 per lane, the next window already in flight), a step is one shuffle + a few integer ops
-// (~40 cycles) and never waits for DRAM; the per-super-k-mer index leaves with coalesced 128-byte stores.
+// and never waits for DRAM; the per-super-k-mer index leaves with coalesced 128-byte stores.
 constexpr int kWalkWarpsPerBlock = 4;
 
 __device__ __forceinline__ uint4 walk_load_window(const uint8_t* bin_aligned, uint64_t wbase, uint64_t limit, uint32_t lane)
@@ -523,7 +523,7 @@ __device__ __forceinline__ uint32_t msd_free_bits(const Rec<WORDS>& r, uint32_t 
 }
 
 // MODE is a template parameter: the bin path (kExpandAll) must not pay registers / shared memory for the oversized-bin modes
-// (measured: with the scatter code in the same instance the kernel went from 32 to more registers and the expansion from 0.75 to 0.90 ms)
+// (with the scatter code in the same instance the kernel needs more than 32 registers and the expansion is slower)
 template <int WORDS, uint32_t MODE = kExpandAll>
 __global__ void __launch_bounds__(ExpandCfg<WORDS>::kThreads, WORDS <= 2 ? 2048 / ExpandCfg<WORDS>::kThreads : 6) expand_kernel(const ExpandArgs a)      // (<= 32 registers for one- and two-word records, <= 42 beyond: the occupancy the kernel was tuned at)
 {

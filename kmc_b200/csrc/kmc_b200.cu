@@ -137,7 +137,7 @@ struct kmcb200_ctx {
 	int occ_leaf_hash = 1;
 	bool leaf_hash_wide = true;                             // KMCB200_LEAF_WIDE = hash | warp: records of more than one word by leaf_hash_wide_kernel / leaf_warp_kernel
 	bool leaf_hash = true;                                  // KMCB200_LEAF_KERNEL = hash | warp: one-word records are counted by leaf_hash_kernel (round 2) / leaf_warp_kernel
-	uint32_t leaf_max_b2 = 9;                               // KMCB200_LEAF_MAX_B2
+	uint32_t leaf_max_b2 = 8;                               // KMCB200_LEAF_MAX_B2 (8: on the H100 the 512 / 1024-digit level 2 costs more than it saves, DESIGN 3.1)
 	uint32_t leaf_target = 1024;                            // KMCB200_LEAF_TARGET: mean leaf size the second partition level of a large bin aims at (leaf_hash_kernel)
 	uint32_t leaf_fill_pct = 62;                            // KMCB200_LEAF_FILL_PCT: leaf_hash_kernel plans a table round for this load
 	uint32_t leaf_ratio0_q8 = 90;                           // KMCB200_LEAF_RATIO0: first guess of distinct k-mers per record, x 256 (30x coverage, 1 % errors: ~0.3)
@@ -148,7 +148,7 @@ struct kmcb200_ctx {
 	uint32_t epoch = 1;
 	uint64_t launches = 0;
 	// All kernels of a context run on ONE stream: the persistent radix passes size their grids to fill the GPU and two of
-	// them side by side only steal SMs from each other (measured: 2.5x slower).  The slots' own streams carry the
+	// them side by side only steal SMs from each other.  The slots' own streams carry the
 	// host<->device copies, so the copies of one bin overlap the kernels of another.
 	cudaStream_t compute = nullptr;
 	std::vector<Slot> slots;
@@ -294,9 +294,8 @@ __global__ void msd_setup_kernel(uint64_t* seg1, uint32_t* item_base1, uint32_t*
 }
 
 // bits of the second partition level.  Counted leaves (the bin path) are streamed by one warp and may be any size: a leaf beyond one
-// table round only costs extra rounds, while the 512 / 1024-digit partition kernels are ~1.3x / 1.7x slower per record than the
-// 256-digit one (measured, B200: 1.2e8 k-mers 3.19 ms with 8 bits vs 3.22 with 9; 2^28 k-mers 7.86 ms with 9 bits vs 8.11 with 10;
-// 2^26 k-mers 1.79 ms with 8 bits vs 1.88 with 9).  So: leaves of ~1 K records while that takes <= 8 bits, then ~2 K-record leaves.
+// table round only costs extra rounds, while the 512 / 1024-digit partition kernels are slower per record than the 256-digit one.
+// So: leaves of ~1 K records while that takes <= 8 bits, then ~2 K-record leaves.
 // Sorted leaves (seam #1) must fit on chip, and canonical k-mers crowd into the low prefixes (largest leaf ~4.4x the mean): aim at a
 // fifth of the capacity, 8 bits at most.
 template <int WORDS>
@@ -307,11 +306,10 @@ uint32_t choose_b2(const kmcb200_ctx* ctx, uint64_t n, bool counted_leaves)
 	if (counted_leaves) {
 		b2 = std::min(bits_for(1024), 10u);
 		// (one-word records only: the leaves of wider records verify every hit against a record in HBM and lose more from a second
-		// table round than the wide scatter costs - k = 55, 2^28 k-mers: 17.1 ms with 10 bits, 21.0 ms with 9)
+		// table round than the wide scatter costs; scripts/l2_bits_sweep.py, DESIGN 3.1)
 		if (WORDS == 1 && b2 > 8 && !ctx->leaf_hash) b2 = std::max(8u, std::min(bits_for(2048), 10u));
 		// leaf_hash_kernel: a leaf of up to ~2100 records of a 30x bin is ONE table round, and the leaves of a bin spread over 0 .. 2x their mean
-		// (measured over the bin sizes of the target workload, profiles/README.md: 9 bits from ~10^8 k-mers on; the 1024-digit count and scatter
-		// kernels cost more than a second table round saves, even at 2^28 k-mers)
+		// (measured over the bin sizes of the target workload with scripts/l2_bits_sweep.py, DESIGN 3.1)
 		if (WORDS == 1 && b2 > 8 && ctx->leaf_hash) b2 = std::max(8u, std::min(bits_for(ctx->leaf_target), ctx->leaf_max_b2));
 		if (ctx->force_b2) b2 = ctx->force_b2;          // (tests: the wide second level on small bins)
 	} else
@@ -461,7 +459,7 @@ int launch_sort(kmcb200_ctx* ctx, Slot& s, void* a, void* b, uint64_t n, uint32_
 			MsdPartArgs p2{};
 			p2.in = b; p2.out = a; p2.items = items2; p2.cell_scan = s.msd_cell_scan; p2.shift = top_shift - b2; p2.nd = nd2;
 			p2.flags = flags;
-			if (nd2 > 256) msd_partition_kernel<WORDS, 1024><<<pgrid2, MsdCfg<WORDS>::kThreads + 32, MsdSmem<WORDS, 1024>::kBytes, st>>>(p2);      // (a 512-digit instance with a third TMA buffer measured slower: 0.61 vs 0.57 ms at 1.2e8 records)
+			if (nd2 > 256) msd_partition_kernel<WORDS, 1024><<<pgrid2, MsdCfg<WORDS>::kThreads + 32, MsdSmem<WORDS, 1024>::kBytes, st>>>(p2);      // (a 512-digit instance with a third TMA buffer was slower)
 			else msd_partition_kernel<WORDS><<<pgrid2, MsdCfg<WORDS>::kThreads + 32, MsdSmem<WORDS>::kBytes, st>>>(p2);
 			ctx->launches++;
 			s.pass_names[iv] = "msd_partition_L2"; CU(cudaEventRecord(s.ev_pass[++iv], st));
@@ -543,7 +541,7 @@ struct ExpandMode {            // oversized bins: count the top 12 bits / keep o
 
 // Host prefix sum of the expander-pack sizes -> pinned staging -> device, on `st`.  The host-buffer path enqueues this on the slot's
 // COPY stream, next to the bin itself: on the compute stream the 8 KB copy would queue up behind the next bin's 66 MB H2D transfer on
-// the same DMA engine and stall the kernels (measured: 0.45 ms per bin).
+// the same DMA engine and stall the kernels.
 int upload_packs(kmcb200_ctx* ctx, Slot& s, uint64_t size, const uint64_t* pack_bytes, uint32_t n_packs, cudaStream_t st)
 {
 	const uint32_t np = (n_packs && pack_bytes) ? n_packs : 1;
@@ -588,7 +586,7 @@ int stage_expand(kmcb200_ctx* ctx, Slot& s, const uint8_t* d_bin, uint64_t size,
 	const uint64_t* pack_bytes, uint32_t n_packs, void* d_recs, cudaStream_t st, const ExpandMode& em = ExpandMode(), bool packs_uploaded = false,
 	uint64_t* zero_lut = nullptr, uint64_t* zero_result = nullptr, cudaStream_t st_walk = nullptr)
 {
-	// st_walk: the slot's copy stream (host-buffer path).  The index of a bin (init + walk + pack scan: ~0.15 ms at 20 % of the SMs, slot-private
+	// st_walk: the slot's copy stream (host-buffer path).  The index of a bin (init + walk + pack scan, slot-private
 	// buffers only) then runs right behind the bin's H2D copy and overlaps the sort / leaves of the bins before it on the compute stream.
 	cudaStream_t st_expand = st;
 	if (st_walk) st = st_walk;
@@ -598,10 +596,10 @@ int stage_expand(kmcb200_ctx* ctx, Slot& s, const uint8_t* d_bin, uint64_t size,
 	const uint32_t np = (n_packs && pack_bytes) ? n_packs : 1;
 	if (!packs_uploaded) if (int rc = upload_packs(ctx, s, size, pack_bytes, n_packs, st)) return rc;
 
-	// ---- KMCB200_EXPAND=fused: one fused pass (expand_fused.cuh) when every pack is a collector flush (<= 64 KiB).  Measured on the B200
-	// (1.2e8 k-mers, k=31): 0.93 ms against 0.80 ms for the index-based kernels below - a lane that walks its own segment executes the
-	// "new record" and the "roll one symbol" paths one after the other (6.0 warp instructions per k-mer against 3.4) - so it is an option
-	// (no per-super-k-mer index in HBM, two launches fewer), not the default.
+	// ---- KMCB200_EXPAND=fused: one fused pass (expand_fused.cuh) when every pack is a collector flush (<= 64 KiB).  Slower than the
+	// index-based kernels below - a lane that walks its own segment executes the "new record" and the "roll one symbol" paths one after
+	// the other (about twice the warp instructions per k-mer) - so it is an option (no per-super-k-mer index in HBM, two launches fewer),
+	// not the default.
 	bool big_pack = !(n_packs && pack_bytes) && size > (uint64_t)kWalkChunk;
 	if (n_packs && pack_bytes) for (uint32_t i = 0; i < n_packs && !big_pack; ++i) big_pack = pack_bytes[i] > (uint64_t)kWalkChunk;
 	const bool fused = ctx->use_fused && !s.have_extras && em.mode == kExpandAll && !big_pack && n_rec != kExpandUnknownRecs && n_rec < (1ull << 32) && n_rec > 0;
@@ -1185,7 +1183,7 @@ int kmcb200_create(const kmcb200_params* prm, kmcb200_ctx** out_ctx)
 	if (prm->device < 0 || prm->device >= n_dev) return fail(ctx, KMCB200_ERR_NO_DEVICE, "device %d not present (%d visible)", prm->device, n_dev);
 	cudaDeviceProp dp;
 	if (cudaGetDeviceProperties(&dp, prm->device) != cudaSuccess) return fail(ctx, KMCB200_ERR_CUDA, "cudaGetDeviceProperties failed");
-	if (dp.major != 10) return fail(ctx, KMCB200_ERR_NO_DEVICE, "device %d is sm_%d%d; kmc_b200 is built for sm_100a only", prm->device, dp.major, dp.minor);
+	if (dp.major != 9 || dp.minor != 0) return fail(ctx, KMCB200_ERR_NO_DEVICE, "device %d is sm_%d%d; kmc_b200 is built for sm_90a (H100) only", prm->device, dp.major, dp.minor);
 
 	ctx = new kmcb200_ctx();
 	ctx->prm = *prm;

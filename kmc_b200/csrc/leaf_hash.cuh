@@ -3,9 +3,9 @@
 //
 // Same job as leaf_warp_kernel (leaf_warp.cuh: the sorted list of a leaf's DISTINCT k-mers with their multiplicities = CompactKmers,
 // kmc_core/kb_sorter.h:1128-1281, fused with the lower levels of the sort), same interface (LeafArgs), same one-warp-per-leaf
-// organisation.  What the profile of leaf_warp_kernel said (profiles/summary_r2f.md, DESIGN 3.2): 7.5 warp instructions per record, of
-// which 41 % in the insertion (the warp iterates its probe loop as often as its unluckiest lane), 25 % in the ring that compacts the
-// k-mers of one of several table rounds - and on the target workload nearly every record sits in a leaf of several rounds, because
+// organisation.  What the profile of leaf_warp_kernel said (DESIGN 3.2): most of its warp instructions went to the insertion (the warp
+// iterates its probe loop as often as its unluckiest lane) and to the ring that compacts the k-mers of one of several table rounds - and
+// on the target workload nearly every record sits in a leaf of several rounds, because
 //   * canonical k-mers are not uniform: the leaf sizes of a bin are spread over 0 .. 2x the mean (the density of canonical k-mers
 //     falls linearly over the key space), and
 //   * the ordered groups of 64 slots overflow long before the table is full: a real k-mer and its ~10 error variants differ in one
@@ -64,8 +64,8 @@ __device__ __forceinline__ uint32_t lh_hash(uint64_t rem) { return ((uint32_t)re
 // Shared-memory atomics on 32-bit shared addresses (inline PTX).  ptxas turns a predicated ATOMS into a branch around it (BSSY / BRA / BSYNC),
 // and those reconvergence points fence the four probe chains of a step off from each other; an UNCONDITIONAL atomic keeps the code
 // straight-line - a lane with nothing to do aims its CAS at a dummy word of its own (holds 0: the compare with EMPTY fails, nothing is written),
-// adds 0 to a count, ORs 0 into a bitmap - but occupies the shared-memory atomic unit for all 32 lanes.  Measured on the B200 (1.17e8-k-mer
-// bin, leaves): everything predicated 0.87 ms, everything unconditional 1.18 ms (the ORs of 32 lanes into a 32-word bitmap collide).
+// adds 0 to a count, ORs 0 into a bitmap - but occupies the shared-memory atomic unit for all 32 lanes, and the ORs of 32 lanes into a
+// 32-word bitmap collide: everything predicated is the faster default.
 #ifndef KMCB200_LH_UNCOND_CAS
 #define KMCB200_LH_UNCOND_CAS 0
 #endif
@@ -238,8 +238,7 @@ __device__ __forceinline__ bool lh_insert(const LhRound& T, const unsigned long 
 		if (!ok) break;
 	}
 	// what is left in the queue at the end of the leaf (< 64 probes): every lane takes one and FOLLOWS it to its slot - a short loop
-	// (a few probes) instead of drain steps that each move a handful of probes by one slot and queue them again (measured: 4.1 such steps
-	// per leaf, 13 % of the kernel's instructions)
+	// (a few probes) instead of drain steps that each move a handful of probes by one slot and queue them again
 	while (ok && tail != head) {
 		__syncwarp();
 		const uint32_t take = min(tail - head, 32u);

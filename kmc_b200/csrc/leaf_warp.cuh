@@ -54,7 +54,7 @@ constexpr uint32_t kLwRing = KMCB200_LW_RING;                // ring of compacte
 constexpr uint32_t kLwMaxLeaf = 65534;           // records of a warp-counted leaf (count field >= 16 bits)
 constexpr uint32_t kLwHeavy = 16384;             // one-word records: a leaf beyond this is first relieved of the copies of ONE dominant k-mer (poly-A,
                                                  // satellite repeats: a k-mer with 10^5..10^6 copies makes its leaf that large); what remains must fit kLwMaxLeaf
-constexpr uint32_t kLwMaxHeavyLeaf = 1u << 22;   // ... and the whole leaf must stay below this (one warp streams it a few times: ~1 ms per 10^6 records)
+constexpr uint32_t kLwMaxHeavyLeaf = 1u << 22;   // ... and the whole leaf must stay below this (one warp streams it a few times)
 constexpr uint32_t kLwMaxSplit = 12;             // extra split bits a round may descend
 constexpr uint64_t kLwEmpty = ~0ull;
 
@@ -219,8 +219,8 @@ __device__ KMCB200_LW_INSERT_ATTR void lw_insert1(const LwRound& t, const uint64
 
 // HEAVY = false: the kernel of the bin path; leaves of one-word records beyond kLwHeavy records are only NOTED (a.heavy_list) and left to a
 // second, tiny launch of the HEAVY = true instance, which knows the dominant-k-mer path.  (With that path compiled into the main instance
-// the common case was 30 % slower - 1.63 ms against 1.24 ms for the leaves of a 1.2e8-k-mer bin: the kernel is that sensitive to registers
-// and code layout - so the main instance stays exactly what it was.)
+// the common case was markedly slower: the kernel is that sensitive to registers and code layout - so the main instance stays exactly
+// what it was.)
 template <int WORDS, int SLOT_BITS, bool HEAVY = false>
 __global__ void __launch_bounds__(32 * kLwWarps, KMCB200_LW_MINBLOCKS) leaf_warp_kernel(const LeafArgs a)
 {

@@ -110,13 +110,11 @@ __device__ __forceinline__ MsdItemGeom msd_item_geom(const MsdItems& it, uint32_
 // dependent global loads: item -> segment -> boundaries), gathers the item's 256 output bases from the cell scan, and fetches the
 // records global->shared with ONE TMA bulk copy into a ring of kStages buffers (full / empty mbarriers).  The consumers never
 // wait for a global load: an item starts when its `full` barrier flips.
-// Measured alternatives (B200, 2^26 8-byte records, per pass): thread 0 claiming tickets and issuing the copies itself, two buffers:
-// 0.272 ms; this pipeline: 0.265 ms; cursors precomputed from the cells by the producer (position = atomicAdd(&cursor[digit], 1)
-// straight into a staging buffer, no histogram / scan, two barriers instead of five): 0.33 ms - fewer instructions, but slower.
-// ncu: the kernel is bound by the shared-memory pipeline (48 % short-scoreboard stalls, ~2100 wavefronts per 4096-record item), not by HBM.
-// Also measured and dropped: the same cursors with in-place regrouping and three buffers (0.39 ms: the single producer warp cannot gather
-// 768 values per item fast enough); loads / atomics / stores of a phase issued in separate batches for more memory-level parallelism
-// (0.29 ms: the pipeline is throughput-, not latency-bound).
+// Tried and dropped: thread 0 claiming tickets and issuing the copies itself; cursors precomputed from the cells by the producer
+// (position = atomicAdd(&cursor[digit], 1) straight into a staging buffer, no histogram / scan, two barriers instead of five) - fewer
+// instructions, but slower; the same cursors with in-place regrouping and three buffers (the single producer warp cannot gather 768
+// values per item fast enough); loads / atomics / stores of a phase issued in separate batches (the pipeline is throughput-, not
+// latency-bound).  The kernel is bound by the shared-memory pipeline, not by HBM.
 // NDMAX = 256 or 1024 digits: the second level of a large bin uses up to 10 bits, so that a leaf still holds ~1 K records
 // (the wider variant has one TMA buffer less: shared memory).
 template <int WORDS, int NDMAX = 256>
@@ -183,7 +181,7 @@ __global__ void __launch_bounds__(MsdCfg<WORDS>::kThreads + 32, MsdCfg<WORDS>::k
 	__syncthreads();
 
 	// items of a CTA: round robin.  (One contiguous block of items per CTA - so that the bases of consecutive items of a digit share sectors
-	// of the cell scan - measured slower on the B200: 0.53 / 0.55 ms against 0.475 / 0.454 for the two passes of a 1.2e8-record bin.)
+	// of the cell scan - was slower.)
 	const uint32_t item_begin = blockIdx.x, item_end = n_items, item_step = gridDim.x;
 	if (tid >= (uint32_t)THREADS) {
 		// ---------------------------------------------------------------- producer warp
@@ -555,7 +553,7 @@ struct MsdLocalArgs {
 	const uint32_t* flags;
 };
 
-// lanes of the warp whose 8-bit digit equals this lane's: 8 ballots (~14 cycles per warp) instead of match.any (32, microcoded; scripts/ubench)
+// lanes of the warp whose 8-bit digit equals this lane's: 8 ballots instead of match.any (microcoded; scripts/ubench measures both)
 __device__ __forceinline__ uint32_t match_digit8(uint32_t d)
 {
 	uint32_t peers = 0xffffffffu;

@@ -5,7 +5,7 @@
 // record image.  Records are pure keys (no payload), so the sorted array is unique and any stable or
 // unstable correct sort is bit-identical to RADULS' output.
 //
-// B200 design: one kernel launch per 8-bit digit, each pass exactly one read + one write of every
+// Design: one kernel launch per 8-bit digit, each pass exactly one read + one write of every
 // record ("onesweep": chained scan with decoupled look-back gives every tile its global bucket
 // offsets inside the same kernel).  Per pass and CTA:
 //   * tiles are fetched global->shared with TMA 1-D bulk copies (cp.async.bulk + mbarrier),

@@ -1,6 +1,6 @@
 """Oversized bins on the hardware (SURVEY 8f N1): one bin of 2^LG k-mers (default 2^31 = 2.1e9 k-mers, 2.2 GB of super-k-mer bytes,
 17 GB of records) through kmcb200_process_bin
-  (a) in one shot - the block limit comes from the free HBM, so a B200 sorts it as ONE bin (one expansion, no key blocks),
+  (a) in one shot - the block limit comes from the free HBM, so a GPU whose free HBM holds it sorts it as ONE bin (one expansion, no key blocks),
   (b) as key blocks of <= 2^(LG-2) k-mers (KMCB200_MAX_BLOCK_RECORDS): one counting expansion + one filtered expansion per block,
       asynchronous block loop, LUT / statistics accumulated on the device,
 and checks that (b) is byte-identical to (a) and that both satisfy the size-independent properties (n_total, sum(LUT) = records,

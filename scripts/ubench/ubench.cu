@@ -1,4 +1,4 @@
-// Micro-benchmarks of the primitives the radix kernels lean on (B200): shared atomics, match.any, ballots, shuffles.
+// Micro-benchmarks of the primitives the radix kernels lean on: shared atomics, match.any, ballots, shuffles.
 // Each test runs ITER dependent-free repetitions per warp on all SMs and reports cycles per warp-instruction per SM-subpartition.
 #include <cstdio>
 #include <cstdint>

@@ -10,7 +10,7 @@ for p in (ROOT, os.path.join(ROOT, "tests")):
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: needs a B200 (run with -m gpu on the GPU box)")
+    config.addinivalue_line("markers", "gpu: needs an H100 (run with -m gpu on a machine that has one)")
 
 
 @pytest.fixture(scope="session")
@@ -18,10 +18,3 @@ def oracle():
     from kmc_testlib import Oracle
     return Oracle()
 
-
-@pytest.fixture(scope="session")
-def reference():
-    from kmc_testlib import Reference, ensure_reference_built
-    if not ensure_reference_built():
-        pytest.skip("oracle/_ref not built and /root/reference absent")
-    return Reference()

@@ -7,6 +7,8 @@
     - `Reference`  : oracle/_ref/libkmc_ref.so       (the unmodified reference classes, when built)
 """
 import ctypes as C
+import hashlib
+import json
 import os
 import subprocess
 from dataclasses import dataclass, field
@@ -19,6 +21,7 @@ ORACLE_SO = os.path.join(ORACLE_DIR, "_build", "libkmc_oracle.so")
 REF_SO = os.path.join(ORACLE_DIR, "_ref", "libkmc_ref.so")
 REF_B200_SO = os.path.join(ORACLE_DIR, "_ref", "libkmc_ref_b200.so")    # same harness, CKmerBinSorterB200 in place of CKmerBinSorter
 PACK_BYTES = 1 << 16          # bin_part_size, kmc_core/kmc.h:151
+REFERENCE_DIGESTS = os.path.join(ROOT, "tests", "golden", "reference_digests.json")    # written by tests/golden/make_reference_digests.py
 
 
 # ----------------------------------------------------------------------------- parameters
@@ -328,6 +331,31 @@ def decode_payload(payload, lut, p: Params):
     return res
 
 
+# ----------------------------------------------------------------------------- stored reference results
+def digest(*arrays):
+    h = hashlib.sha256()
+    for a in arrays:
+        h.update(a if isinstance(a, bytes) else np.ascontiguousarray(a).tobytes())
+    return h.hexdigest()
+
+
+def bin_digest(b):
+    """Identifies a generated input: a golden digest is only meaningful for the bin it was computed from."""
+    return digest(np.ascontiguousarray(b.data, dtype=np.uint8), np.ascontiguousarray(b.pack_bytes, dtype=np.uint64))
+
+
+def result_digest(r):
+    """A stage-2 result (payload, LUT, the four counters) in the form the stored reference results take."""
+    payload = r.payload if isinstance(r.payload, bytes) else r.payload.tobytes()
+    return {"payload": digest(payload), "lut": digest(np.asarray(r.lut, dtype=np.uint64)), "stats": [int(x) for x in r.stats]}
+
+
+def reference_digest(case):
+    """What the unmodified reference computed for `case` (input digest + result digests), stored when the fixture was made."""
+    with open(REFERENCE_DIGESTS) as f:
+        return json.load(f)[case]
+
+
 # ----------------------------------------------------------------------------- build helpers
 def ensure_oracle_built():
     src = os.path.join(ORACLE_DIR, "stage2_oracle.c")
@@ -341,9 +369,10 @@ def reference_available():
 
 
 def ensure_reference_built():
-    """Build oracle/_ref from /root/reference when it is there (dev container); on the GPU box the prebuilt .so travels."""
-    if not os.path.exists(REF_SO) and os.path.exists("/root/reference/kmc_core/kb_sorter.h"):
-        subprocess.check_call(["make", "-C", ORACLE_DIR, "ref"], stdout=subprocess.DEVNULL)
+    """Build oracle/_ref when it is missing (oracle/Makefile: from the KMC source tree REF, or KMC_REFERENCE_DIR; a no-op without one)."""
+    if not os.path.exists(REF_SO):
+        ref = ["REF=" + os.path.abspath(os.environ["KMC_REFERENCE_DIR"])] if os.environ.get("KMC_REFERENCE_DIR") else []
+        subprocess.check_call(["make", "-C", ORACLE_DIR, "ref"] + ref, stdout=subprocess.DEVNULL)
     return os.path.exists(REF_SO)
 
 
@@ -437,7 +466,7 @@ class Reference:
 
     def __init__(self, with_b200=False):
         if not ensure_reference_built():
-            raise RuntimeError("oracle/_ref/libkmc_ref.so is not built and /root/reference is absent")
+            raise RuntimeError("oracle/_ref/libkmc_ref.so is not built (make -C oracle ref [REF=<KMC source tree>])")
         if with_b200 and not os.path.exists(REF_B200_SO):
             raise RuntimeError("oracle/_ref/libkmc_ref_b200.so is not built")
         self.lib = C.CDLL(REF_B200_SO if with_b200 else REF_SO)

@@ -1,16 +1,30 @@
 """The database writer of SURVEY 8f N3 (kmcb200_db_*: pinned staging ring, writer thread, footer) against files written by the REFERENCE:
-a database made by the unmodified reference CLI (oracle/_ref/kmc_ref, one stage-2 sorter so that the bin order is deterministic) is taken
-apart into its bins (payload and LUT of every bin, signature map, header fields) and replayed through the writer; .kmc_pre and .kmc_suf must
-come out byte for byte.  Host-only: runs without a GPU (the staging ring is then plain memory)."""
+a database made by the unmodified reference CLI (one stage-2 sorter so that the bin order is deterministic; stored in
+tests/golden/refdb_k*.npz by tests/golden/make_reference_digests.py) is taken apart into its bins (payload and LUT of every bin, signature
+map, header fields) and replayed through the writer; .kmc_pre and .kmc_suf must come out byte for byte.  Host-only: runs without a GPU
+(the staging ring is then plain memory)."""
 import os
 import struct
 
 import numpy as np
 import pytest
 
-from test_gpu_kmc_files import KMC_REF, write_fastq, count
-
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
+GOLD = os.path.join(ROOT, "tests", "golden")
+# the reference CLI's runs behind tests/golden/refdb_k<k>.npz: 200 reads of tests/test_gpu_kmc_files.write_fastq(seed 500 + k,
+# genome_len=2000, err=0.002), `kmc -k<k> -fq -m2 -t4 -sr1 -n64 <extra>`
+REFDB_CASES = {31: ("-ci2",), 28: ("-ci1", "-cs65535"), 55: ("-ci1", "-b")}
+REFDB_STATS = ("#Unique_k-mers", "#k-mers_below_min_threshold", "#k-mers_above_max_threshold", "#Total no. of k-mers")
+
+
+def load_reference_db(k, tmp):
+    """The stored reference database of REFDB_CASES[k] as <tmp>/ref.kmc_pre / .kmc_suf, and its statistics."""
+    z = np.load(os.path.join(GOLD, "refdb_k%d.npz" % k))
+    db = os.path.join(tmp, "ref")
+    for ext in ("kmc_pre", "kmc_suf"):
+        with open(db + "." + ext, "wb") as f:
+            f.write(z[ext].tobytes())
+    return db, dict(zip(REFDB_STATS, (int(x) for x in z["stats"])))
 
 
 def parse_db(prefix):
@@ -38,21 +52,16 @@ def parse_db(prefix):
                 sig_map=sig_map, luts=luts, payloads=payloads, n_recs=n_recs)
 
 
-@pytest.mark.parametrize("k,extra", [(31, ("-ci2",)), (28, ("-ci1", "-cs65535")), (55, ("-ci1", "-b"))])
+@pytest.mark.parametrize("k,extra", list(REFDB_CASES.items()))
 @pytest.mark.parametrize("raw_lut", [False, True])
 def test_writer_reproduces_reference_files(tmp_path, k, extra, raw_lut):
     import ctypes as C
     import kmc_b200
-    if not os.path.exists(KMC_REF):
-        pytest.skip("oracle/_ref/kmc_ref not built")
     tmp = str(tmp_path)
-    fq = os.path.join(tmp, "reads.fq")
-    write_fastq(fq, 500 + k, 8000)
-    db, stats = count(KMC_REF, tmp, "ref", fq, k, extra + ("-sr1", "-n64"))
+    db, st = load_reference_db(k, tmp)
     d = parse_db(db)
-    st = stats["Stats"]
     out = os.path.join(tmp, "replay")
-    w = kmc_b200.DbWriter(out, d["k"], d["counter_size"], d["p"], d["sig_len"], d["cmin"], d["cmax"], d["both"], staging_bytes=1 << 20)   # a small ring: it wraps and blocks
+    w = kmc_b200.DbWriter(out, d["k"], d["counter_size"], d["p"], d["sig_len"], d["cmin"], d["cmax"], d["both"], staging_bytes=1 << 20)   # the smallest ring (1 MB); the standalone tests below make it wrap
     n_bins = d["luts"].shape[0]
     for b in range(n_bins):
         pay = d["payloads"][b]
@@ -74,8 +83,42 @@ def test_writer_reproduces_reference_files(tmp_path, k, extra, raw_lut):
 
 def _standalone_bins():
     from kmc_testlib import synth_bin
-    sizes = [4000, 0, 900, 15000, 1, 7000]
+    sizes = [4000, 0, 900, 15000, 1, 7000, 200000]          # the last bin alone emits > 1 MB of records: the 1 MB staging ring wraps and blocks
     return [synth_bin(40 + i, 31, n, genome_len=max(n, 500)) for i, n in enumerate(sizes)]
+
+
+RING_BYTES = 1 << 20                # kmcb200_db_open's smallest staging ring (db_writer.inl), what the tests below ask for
+
+
+def write_standalone(out, results, p):
+    """Oracle results -> the writer (raw LUTs, bin i holds signature i) -> out.kmc_pre / out.kmc_suf; returns the totals."""
+    import ctypes as C
+    import kmc_b200
+    w = kmc_b200.DbWriter(out, p.k, p.counter_bytes, p.lut_prefix_len, 9, p.cutoff_min, p.cutoff_max, True, staging_bytes=RING_BYTES)
+    for i, r in enumerate(results):
+        ptr = w.reserve(len(r.payload))
+        C.memmove(ptr, r.payload, len(r.payload))
+        w.commit_bin(len(r.payload), r.lut, r.stats, [i], raw_lut=True)
+    return w.close()
+
+
+def db_digest(prefix):
+    from kmc_testlib import digest
+    return {ext: digest(open(prefix + ext, "rb").read()) for ext in (".kmc_pre", ".kmc_suf")}
+
+
+def _assert_reference_readable(out, case, results, p):
+    """The files are byte for byte the ones the reference's kmc_tools read back to the expected dump when the digests were stored
+    (tests/golden/make_reference_digests.py), and this file's reader decodes them to the same dump."""
+    from kmc_testlib import reference_digest, decode_payload
+    assert db_digest(out) == reference_digest(case)["results"]["kmc_tools_read_back"]
+    d = parse_db(out)
+    ends = np.append(d["luts"][1:, 0], np.uint64(d["n_recs"]))
+    decoded = []
+    for b, pay in enumerate(d["payloads"]):
+        counts = np.diff(np.append(d["luts"][b], ends[b]).astype(np.int64))
+        decoded += ["%s\t%d" % (s, c) for s, c in decode_payload(pay, counts, p)]
+    assert decoded == _expected_dump(results, p)
 
 
 def _expected_dump(results, p):
@@ -87,27 +130,15 @@ def _expected_dump(results, p):
 
 
 def test_standalone_database_is_readable_by_the_reference_tools(tmp_path, oracle):
-    """Bins -> (oracle results) -> writer -> files; the reference's kmc_tools must read the database back bin after bin."""
-    import ctypes as C
-    import kmc_b200
+    """Bins -> (oracle results) -> writer -> files that the reference's kmc_tools reads back bin after bin."""
     from kmc_testlib import Params
-    from test_gpu_kmc_files import KMC_TOOLS, run
-    if not os.path.exists(KMC_TOOLS):
-        pytest.skip("oracle/_ref/kmc_tools not built")
     p = Params(k=31, cutoff_min=2, lut_prefix_len=7)
-    bins = _standalone_bins()
-    res = [oracle.process_bin(b, p) for b in bins]
+    res = [oracle.process_bin(b, p) for b in _standalone_bins()]
     out = os.path.join(str(tmp_path), "standalone")
-    w = kmc_b200.DbWriter(out, 31, p.counter_bytes, 7, 9, p.cutoff_min, p.cutoff_max, True, staging_bytes=1 << 20)
-    for i, r in enumerate(res):
-        ptr = w.reserve(len(r.payload))
-        C.memmove(ptr, r.payload, len(r.payload))
-        w.commit_bin(len(r.payload), r.lut, r.stats, [i], raw_lut=True)
-    tot = w.close()
+    assert sum(len(r.payload) for r in res) > RING_BYTES
+    tot = write_standalone(out, res, p)
     assert tot == tuple(sum(r.stats[j] for r in res) for j in range(4))
-    txt = os.path.join(str(tmp_path), "dump.txt")
-    run([KMC_TOOLS, "transform", out, "dump", txt])
-    assert open(txt).read().split("\n")[:-1] == _expected_dump(res, p)
+    _assert_reference_readable(out, "standalone_db", res, p)
 
 
 @pytest.mark.gpu
@@ -116,15 +147,12 @@ def test_gpu_bins_straight_into_the_database(tmp_path, oracle):
     sum on the GPU, base = records so far) -> commit; two bins in flight while the writer thread appends the earlier ones."""
     import kmc_b200
     from kmc_testlib import Params
-    from test_gpu_kmc_files import KMC_TOOLS, run
-    if not os.path.exists(KMC_TOOLS):
-        pytest.skip("oracle/_ref/kmc_tools not built")
     p = Params(k=31, cutoff_min=2, lut_prefix_len=7)
     bins = _standalone_bins() * 3
     res = [oracle.process_bin(b, p) for b in bins]
     out = os.path.join(str(tmp_path), "gpu_db")
     ctx = kmc_b200.Stage2Context(kmc_b200.Stage2Params(31, True, 2, 10 ** 9, 255, 7), device=0, n_slots=2)
-    w = kmc_b200.DbWriter(out, 31, p.counter_bytes, 7, 9, p.cutoff_min, p.cutoff_max, True, staging_bytes=1 << 18)
+    w = kmc_b200.DbWriter(out, 31, p.counter_bytes, 7, 9, p.cutoff_min, p.cutoff_max, True, staging_bytes=RING_BYTES)
     luts = [np.zeros(ctx.lut_entries, dtype=np.uint64) for _ in range(2)]
     datas = [np.ascontiguousarray(b.data) for b in bins]
 
@@ -143,6 +171,4 @@ def test_gpu_bins_straight_into_the_database(tmp_path, oracle):
     tot = w.close()
     ctx.close()
     assert tot == tuple(sum(r.stats[j] for r in res) for j in range(4))
-    txt = os.path.join(str(tmp_path), "dump.txt")
-    run([KMC_TOOLS, "transform", out, "dump", txt])
-    assert open(txt).read().split("\n")[:-1] == _expected_dump(res, p)
+    _assert_reference_readable(out, "standalone_db_x3", res, p)

@@ -8,8 +8,8 @@ completer, file format - the reference's unchanged code), against the unmodified
   L2  `kmc_tools transform db dump -s` text identical, also with several GPU sorter objects (any completion order)
   +   the reference's CLI known-answers (.github/workflows/main.yml:35-52; the reads live in tests/golden/kats.json)
 
-The binaries are built in the dev container by `make -C oracle cli` (oracle/Makefile) and travel to the GPU box; nothing here reads
-/root/reference at run time.
+The binaries are built from a KMC source tree by `make -C oracle cli REF=<tree>` (or build() with KMC_REFERENCE_DIR=<tree>); without
+them these tests skip.  Nothing here reads the KMC sources at run time.
 """
 import hashlib
 import json
@@ -29,7 +29,7 @@ KMC_REF, KMC_B200, KMC_TOOLS = (os.path.join(REF, n) for n in ("kmc_ref", "kmc_b
 def _need_binaries():
     for b in (KMC_REF, KMC_B200, KMC_TOOLS):
         if not os.path.exists(b):
-            pytest.skip("%s not built (make -C oracle cli needs /root/reference)" % os.path.basename(b))
+            pytest.skip("%s not built (make -C oracle cli REF=<KMC source tree>)" % os.path.basename(b))
 
 
 def write_fastq(path, seed, n_reads, read_len=150, genome_len=200_000, err=0.01, n_frac=0.002):

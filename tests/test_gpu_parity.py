@@ -354,46 +354,45 @@ def test_leaf_count_crowded_leaf_and_heavy_kmer(oracle):
 
 
 # ----------------------------------------------------------------------------------------------------------------------
-# Round 2: parity at benchmark scale, against the reference itself (oracle/_ref/libkmc_ref.so travels to the GPU box)
-def _reference_or_skip():
-    from kmc_testlib import Reference, reference_available
-    if not reference_available():
-        pytest.skip("oracle/_ref/libkmc_ref.so not built")
-    return Reference()
+# Parity at benchmark scale, against what the unmodified CKmerBinSorter<SIZE>::ProcessBins + RADULS computed on the same bins
+# (tests/golden/reference_digests.json, made by tests/golden/make_reference_digests.py)
+LARGE_BINS = {"bench_scale_k31": (31, 7, 2600 + 31, 1 << 26), "bench_scale_k55": (55, 7, 2600 + 55, 1 << 26), "large_second_level_k31": (31, 7, 117, 117_000_000)}
 
 
-def _assert_same(r, e, what=""):
-    assert r.stats == tuple(e.stats), what
-    assert np.array_equal(r.lut, e.lut), what
-    assert r.payload.tobytes() == e.payload, what
+def large_bin(case):
+    k, p_len, seed, n = LARGE_BINS[case]
+    return Params(k=k, cutoff_min=2, lut_prefix_len=p_len), fast_bin(seed, k, n)
+
+
+def _assert_reference(r, b, case):
+    from kmc_testlib import bin_digest, result_digest, reference_digest
+    exp = reference_digest(case)
+    assert bin_digest(b) == exp["input"], "%s: the generated bin is not the one the reference result was stored for" % case
+    assert result_digest(r) == exp["results"]["raduls"], case
 
 
 @pytest.mark.parametrize("k,p_len", [(31, 7), (55, 7)])
 def test_benchmark_scale_bit_exact_vs_reference(k, p_len):
     """One bin of 2^26 k-mers (BASELINE configs[1] / the benchmark's bin size): payload, LUT and statistics byte for byte
     against the unmodified CKmerBinSorter<SIZE>::ProcessBins + RADULS (k=55: against the reference's (k,x)-mer path)."""
-    import os
-    R = _reference_or_skip()
-    p = Params(k=k, cutoff_min=2, lut_prefix_len=p_len)
-    b = fast_bin(2600 + k, k, 1 << 26)
+    p, b = large_bin("bench_scale_k%d" % k)
     ctx = _ctx(p)
     r = ctx.process_bin(b)
-    e = R.process_bin(b, p, n_sorters=os.cpu_count() or 8)
-    _assert_same(r, e, "k=%d" % k)
+    _assert_reference(r, b, "bench_scale_k%d" % k)
     assert r.n_total == 1 << 26
     ctx.close()
 
 
-def test_large_second_level_bit_exact_vs_reference():
-    """A bin of the target workload's size (1.2e8 k-mers: 9-bit second partition level, 2^17 leaves) against the reference."""
-    import os
-    R = _reference_or_skip()
-    p = Params(k=31, cutoff_min=2, lut_prefix_len=7)
-    b = fast_bin(117, 31, 117_000_000)
-    ctx = _ctx(p)
-    r = ctx.process_bin(b)
-    _assert_same(r, R.process_bin(b, p, n_sorters=os.cpu_count() or 8))
-    ctx.close()
+def test_large_second_level_bit_exact_vs_reference(monkeypatch):
+    """A bin of the target workload's size (1.2e8 k-mers) against the reference: the default second partition level (8 bits, leaves of
+    ~1.8 K records) and a forced 9-bit one (512-digit count and scatter, 2^17 leaves)."""
+    p, b = large_bin("large_second_level_k31")
+    for bits in (None, "9"):
+        if bits:
+            monkeypatch.setenv("KMCB200_L2_BITS", bits)
+        ctx = _ctx(p)
+        _assert_reference(ctx.process_bin(b), b, "large_second_level_k31")
+        ctx.close()
 
 
 def _golden():

@@ -94,6 +94,7 @@ int kmcb200_host_free(kmcb200_ctx* ctx, void* ptr);
  *   n_plus_x_recs   : (k+x)-mer estimate; accepted for signature parity, unused (we never build (k,x)-mers)
  *   pack_bytes[n_packs] : byte length of every expander pack (CExpanderPackDesc, first of each pair,
  *                     queues.h:376-396); packs start on record boundaries.  pack_recs may be NULL (unused).
+ *                     A pack may have 0 bytes or more than 64 KiB (the latter is walked by one warp instead of one CTA).
  * Outputs = what is handed to kq->push (kb_sorter.h:1273, queues.h:826):
  *   out_suffix[0, *out_bytes) : the emitted records (one data pack (0, out_pos))
  *   lut[4^p]                  : raw per-prefix counts (the completer does the prefix sum)

@@ -38,6 +38,9 @@ def main():
     for cmin, cmax, cntmax in T.CUTOFF_CASES:
         p, b = T.cutoff_case(cmin, cmax, cntmax)
         one("cutoff_ci%d_cx%d_cs%d" % (cmin, cmax, cntmax), b, p, {"raduls": {}})
+    for case in sorted(T.CORNER_CASES):
+        p, b = T.corner_case(case)
+        one(case, b, p, {"raduls": {}})
     for i, b in enumerate(T.edge_bins()):
         one("edge_%d" % i, b, Params(k=31, cutoff_min=1, lut_prefix_len=7), {"raduls": {}})
     p = Params(k=31, cutoff_min=2, lut_prefix_len=7)

@@ -14,6 +14,12 @@ REF_VARIANTS = {"raduls": dict(), "radix_h": dict(sort_kind=1), "raduls_4_sorter
 CUTOFF_CASES = [(1, 10 ** 9, 255), (3, 9, 4), (2, 300, 65535), (1, 10 ** 9, 1)]
 SORT_CASES = [(1, 8), (1, 5), (2, 14), (2, 15), (3, 18), (4, 32)]
 SEVERAL_SIZES = [400, 0, 2500, 30, 1200]
+# corners of the record and counter layout: k = 65 / 97 (the first k of 3- and 4-word records: the top symbols sit in the low bits of a
+# fresh word), 4-byte counters with a count in the third byte, counter_max = 1 with wide records, cutoff_max setting the counter width, and
+# p = 15 (a 4^15-entry LUT, with a small bin).  name: (k, both_strands, cutoff_min, cutoff_max, counter_max, lut_prefix_len, copies of one k-mer)
+CORNER_CASES = {"corner_k65_cs4": (65, True, 1, 10 ** 9, 2 ** 32 - 1, 5, 70000), "corner_k97_cs3": (97, False, 2, 10 ** 9, 2 ** 24 - 1, 5, 0),
+                "corner_k55_cs1": (55, True, 1, 10 ** 9, 1, 7, 0), "corner_k31_cs4_cx200": (31, True, 1, 200, 2 ** 32 - 1, 7, 300),
+                "corner_k127_p15": (127, True, 1, 10 ** 9, 65535, 15, 0)}
 
 
 def bin_case(k, both, cmin):
@@ -32,6 +38,15 @@ def edge_bins():
             pack_superkmers(31, [rng.integers(0, 4, 31 + 255) for _ in range(40)]),
             pack_superkmers(31, [np.zeros(31 + 255, dtype=np.uint8) for _ in range(30)]),
             pack_superkmers(31, [np.tile(np.array([0, 3], dtype=np.uint8), 100)[:31 + 150] for _ in range(20)])]
+
+
+def corner_case(case):
+    k, both, cmin, cmax, cntmax, p_len, copies = CORNER_CASES[case]
+    rng = np.random.default_rng(900 + k + copies)
+    genome = rng.integers(0, 4, 640 + k)
+    starts, lens = rng.integers(0, 600, 1500), k + rng.integers(0, 40, 1500)
+    lists = [genome[s:s + n] for s, n in zip(starts, lens)] + [genome[:k]] * copies
+    return Params(k=k, both_strands=both, cutoff_min=cmin, cutoff_max=cmax, counter_max=cntmax, lut_prefix_len=p_len), pack_superkmers(k, lists)
 
 
 def several_bins():
@@ -65,6 +80,12 @@ def test_cutoffs_and_clamp_match_reference(oracle):
     for cmin, cmax, cntmax in CUTOFF_CASES:
         p, b = cutoff_case(cmin, cmax, cntmax)
         _check(oracle.process_bin(b, p), "cutoff_ci%d_cx%d_cs%d" % (cmin, cmax, cntmax), b)
+
+
+@pytest.mark.parametrize("case", sorted(CORNER_CASES))
+def test_corners_match_reference(oracle, case):
+    p, b = corner_case(case)
+    _check(oracle.process_bin(b, p), case, b)
 
 
 def test_edge_bins_match_reference(oracle):

@@ -156,6 +156,59 @@ int kmcb200_db_commit_bin(kmcb200_db_writer* w, uint64_t payload_bytes, const ui
 	const uint32_t* signatures, uint32_t n_signatures);
 int kmcb200_db_close(kmcb200_db_writer* w, uint64_t totals[4]);
 
+/* ---- stage 1: reads -> bins (SURVEY 8f N4: GPU super-k-mer splitting) -------------------------------------------------------------
+ * The work of CSplitter::ProcessReads (kmc_core/splitter.cpp:557-677) and CKmerBinCollector::PutExtendedKmer (kb_collector.cpp:34-90) for
+ * one batch of sequences, on the GPU.  A batch is one byte array: ACGTacgt are bases (splitter.cpp:43-47), every other byte ends the
+ * current N-free segment, so reads are simply joined with one separator byte (e.g. '\n') between them.  Each sequence is treated as one
+ * unsplit read (the reference cuts reads longer than mem_part_pmm_reads into overlapping parts, splitter.cpp:143-169: that adds
+ * super-k-mer cuts but moves no k-mer to another bin).
+ * Output: the bins' byte streams concatenated in bin order, the expander packs of all bins in bin order, and one fragment per bin.  Inside
+ * a bin the records are in input order, byte for byte the stream of the reference run with one splitter thread.  In one batch's fragment
+ * of a bin, the record that starts at byte s belongs to pack s / 65408: every pack starts on a record boundary, is non-empty and holds at
+ * most 65536 bytes (so stage 2 walks every pack with one CTA).  A bin's stream over several batches is the concatenation of its fragments
+ * in batch order, and so is its pack list; cut between reads, any batching gives the same bins as one batch.
+ * The signature map is what CSignatureMapper::get_bin_id reads (s_mapper.h:263-266): 4^signature_len + 1 entries, the last one for the
+ * special signature; every entry must be below n_bins.  A map read from a .kmc_pre (kb_completer.cpp:211-221, file positions of the bins)
+ * reproduces the reference's file order when the bins are committed in order 0..n_bins-1.
+ * The HBM workspace is allocated by kmcb200_splitter_create from max_batch_bytes (DESIGN.md section 3.8 gives its bytes per base).  Create
+ * the splitter before the stage-2 contexts of the same GPU: kmcb200_create sizes its block limit from the HBM that is free at that moment. */
+#define KMCB200_SPLIT_MAX_BINS 4096
+#define KMCB200_SPLIT_MAX_BATCH (1ull << 31)
+typedef struct kmcb200_splitter kmcb200_splitter;
+typedef struct {
+	uint32_t kmer_len;                    /* Params.kmer_len: signature_len+1 .. KMCB200_MAX_KMER_LEN */
+	uint32_t signature_len;               /* Params.signature_len (-p): 5..11 */
+	uint32_t n_bins;                      /* 1..KMCB200_SPLIT_MAX_BINS; every map value is < n_bins (the special signature maps like any other) */
+	int32_t device;                       /* CUDA ordinal */
+	uint64_t max_batch_bytes;             /* largest batch one call accepts (1..KMCB200_SPLIT_MAX_BATCH): sizes the workspace */
+} kmcb200_split_params;
+typedef struct {
+	uint64_t byte_off;                    /* offset of the bin's bytes in the output */
+	uint64_t bytes;                       /* size of the bin's stream in this batch */
+	uint64_t n_rec;                       /* k-mers (CBinDesc n_rec, kb_collector.cpp:74) */
+	uint64_t n_super_kmers;               /* records */
+	uint32_t pack0, n_packs;              /* the bin's packs: pack_bytes[pack0 .. pack0 + n_packs) */
+} kmcb200_bin_fragment;
+
+/* KMCB200_ERR_INVALID for a bad parameter or a map value >= n_bins, KMCB200_ERR_NO_DEVICE without an sm_90 device (no CPU fallback). */
+int kmcb200_splitter_create(const kmcb200_split_params* params, const uint32_t* signature_map /* host, 4^signature_len + 1 */, kmcb200_splitter** out);
+void kmcb200_splitter_destroy(kmcb200_splitter* sp);
+/* message of the last failure on this splitter (or of the last failed kmcb200_splitter_create when sp == NULL) */
+const char* kmcb200_splitter_last_error(const kmcb200_splitter* sp);
+/* Host buffers: copies the batch in and returns when out[0, *out_bytes), pack_bytes[0, *n_packs) and frags[n_bins] are filled.  When
+ * out_capacity or pack_capacity is too small: KMCB200_ERR_CAPACITY, *out_bytes / *n_packs give the required sizes, nothing else is written. */
+int kmcb200_split(kmcb200_splitter* sp, const uint8_t* seq, uint64_t bytes,
+	uint8_t* out, uint64_t out_capacity, uint64_t* out_bytes,
+	uint64_t* pack_bytes, uint64_t pack_capacity, uint64_t* n_packs, kmcb200_bin_fragment* frags);
+/* Device twin: every pointer is a device pointer, the work is queued on `stream` (a cudaStream_t; NULL = the legacy default stream).
+ * d_result receives 5 x uint64: [0] output bytes, [1] packs, [2] 1 when a capacity was too small (then only d_result is written: the
+ * required sizes), [3] records (super-k-mers), [4] k-mers.  d_frags[n_bins] as in kmcb200_split.  Stage 2's device entry points read a
+ * bin 32 bytes past its end: give d_out that much slack when its bins go to kmcb200_dev_process_bin in place. */
+int kmcb200_dev_split(kmcb200_splitter* sp, const uint8_t* d_seq, uint64_t bytes, uint8_t* d_out, uint64_t out_capacity,
+	uint64_t* d_pack_bytes, uint64_t pack_capacity, kmcb200_bin_fragment* d_frags, uint64_t* d_result, void* stream);
+/* Number of kernels this splitter has launched so far. */
+uint64_t kmcb200_splitter_kernel_launches(const kmcb200_splitter* sp);
+
 /* ---- seam #1: sort host records ------------------------------------------------------------------
  * Contract of SortFunction (raduls.h:19-20, kb_sorter.h:775-779): n records of rec_bytes (multiple of 8,
  * CKmer<SIZE> images) sorted ascending on bytes key_bytes-1..0; the result is left in `tmp` when key_bytes

@@ -35,12 +35,24 @@ class _DbParams(C.Structure):
                 ("cutoff_min", C.c_uint32), ("cutoff_max", C.c_uint32), ("both_strands", C.c_uint32)]
 
 
+class _SplitParams(C.Structure):
+    _fields_ = [("kmer_len", C.c_uint32), ("signature_len", C.c_uint32), ("n_bins", C.c_uint32), ("device", C.c_int32), ("max_batch_bytes", C.c_uint64)]
+
+
+class BinFragment(C.Structure):
+    """kmcb200_bin_fragment: one bin's share of a split batch."""
+    _fields_ = [("byte_off", C.c_uint64), ("bytes", C.c_uint64), ("n_rec", C.c_uint64), ("n_super_kmers", C.c_uint64),
+                ("pack0", C.c_uint32), ("n_packs", C.c_uint32)]
+
+
 EXPORTS = [
     "kmcb200_create", "kmcb200_destroy", "kmcb200_last_error", "kmcb200_out_rec_bytes", "kmcb200_out_capacity", "kmcb200_lut_entries",
     "kmcb200_host_alloc", "kmcb200_host_free", "kmcb200_process_bin", "kmcb200_process_bin_multi", "kmcb200_submit_bin", "kmcb200_submit_bin_indexed", "kmcb200_wait_bin", "kmcb200_sort_records",
     "kmcb200_dev_process_bin", "kmcb200_dev_expand", "kmcb200_dev_sort", "kmcb200_dev_count", "kmcb200_kernel_launches",
     "kmcb200_stage_times", "kmcb200_stage_names",
     "kmcb200_wait_bin_scanned", "kmcb200_db_open", "kmcb200_db_last_error", "kmcb200_db_records", "kmcb200_db_reserve", "kmcb200_db_commit_bin", "kmcb200_db_close",
+    "kmcb200_splitter_create", "kmcb200_splitter_destroy", "kmcb200_splitter_last_error", "kmcb200_split", "kmcb200_dev_split",
+    "kmcb200_splitter_kernel_launches",
 ]
 
 _lib = None
@@ -93,6 +105,15 @@ def load_library(build_if_needed=True):
     L.kmcb200_db_reserve.argtypes = [vp, u64, C.POINTER(vp)]
     L.kmcb200_db_commit_bin.argtypes = [vp, u64, vp, C.c_int, vp, vp, u32]
     L.kmcb200_db_close.argtypes = [vp, vp]
+    L.kmcb200_splitter_create.argtypes = [C.POINTER(_SplitParams), vp, C.POINTER(vp)]
+    L.kmcb200_splitter_destroy.argtypes = [vp]
+    L.kmcb200_splitter_destroy.restype = None
+    L.kmcb200_splitter_last_error.argtypes = [vp]
+    L.kmcb200_splitter_last_error.restype = C.c_char_p
+    L.kmcb200_split.argtypes = [vp, vp, u64, vp, u64, C.POINTER(u64), vp, u64, C.POINTER(u64), vp]
+    L.kmcb200_dev_split.argtypes = [vp, vp, u64, vp, u64, vp, u64, vp, vp, vp]
+    L.kmcb200_splitter_kernel_launches.argtypes = [vp]
+    L.kmcb200_splitter_kernel_launches.restype = u64
     _lib = L
     return L
 
@@ -306,3 +327,76 @@ class DbWriter:
         if rc != 0:
             raise KmcB200Error(rc, "kmcb200_db_close")
         return tuple(int(x) for x in tot)
+
+
+class Splitter:
+    """Stage 1 on one GPU (kmcb200_splitter_*): batches of sequences -> KMC bins (CSplitter::ProcessReads, kmc_core/splitter.cpp:557-677).
+
+    A batch is one byte array in which every byte other than ACGTacgt separates (reads.sequences_to_batch makes one from FASTQ / FASTA).
+    `signature_map` has 4^signature_len + 1 entries, each below n_bins."""
+
+    def __init__(self, kmer_len, signature_len, signature_map, n_bins=None, device=0, max_batch_bytes=1 << 26):
+        self.lib = load_library()
+        sig_map = np.ascontiguousarray(signature_map, dtype=np.uint32)
+        if sig_map.size != (1 << (2 * signature_len)) + 1:
+            raise KmcB200Error(ERR_INVALID, "signature_map has %d entries, 4^%d + 1 expected" % (sig_map.size, signature_len))
+        self.n_bins = int(sig_map.max()) + 1 if n_bins is None else int(n_bins)
+        self.kmer_len, self.signature_len, self.max_batch_bytes = kmer_len, signature_len, max_batch_bytes
+        self._h = C.c_void_p(None)
+        p = _SplitParams(kmer_len, signature_len, self.n_bins, device, max_batch_bytes)
+        rc = self.lib.kmcb200_splitter_create(C.byref(p), sig_map.ctypes.data, C.byref(self._h))
+        if rc != 0:
+            raise KmcB200Error(rc, (self.lib.kmcb200_splitter_last_error(None) or b"").decode())
+        self._out = np.empty(0, dtype=np.uint8)
+        self._packs = np.empty(0, dtype=np.uint64)
+
+    def _check(self, rc):
+        if rc < 0:
+            raise KmcB200Error(rc, (self.lib.kmcb200_splitter_last_error(self._h) or b"").decode())
+        return rc
+
+    def close(self):
+        if self._h:
+            self.lib.kmcb200_splitter_destroy(self._h)
+            self._h = C.c_void_p(None)
+
+    def __del__(self):
+        try:
+            self.close()
+        except Exception:
+            pass
+
+    def kernel_launches(self):
+        return int(self.lib.kmcb200_splitter_kernel_launches(self._h))
+
+    def split_raw(self, batch, out=None, pack_bytes=None):
+        """kmcb200_split into the given (or internal, grown as needed) buffers: (out[:bytes], pack_bytes[:n_packs], fragments)."""
+        seq = np.ascontiguousarray(np.frombuffer(batch, dtype=np.uint8) if isinstance(batch, (bytes, bytearray)) else batch, dtype=np.uint8)
+        frags = (BinFragment * self.n_bins)()
+        nbytes, npacks = C.c_uint64(0), C.c_uint64(0)
+        own = out is None
+        for _ in range(2):
+            o = self._out if own else out
+            pk = self._packs if pack_bytes is None else pack_bytes
+            rc = self.lib.kmcb200_split(self._h, seq.ctypes.data, seq.size, o.ctypes.data, o.size, C.byref(nbytes),
+                                        pk.ctypes.data, pk.size, C.byref(npacks), frags)
+            if rc == ERR_CAPACITY and own and pack_bytes is None:
+                self._out = np.empty(int(nbytes.value * 1.25) + 1024, dtype=np.uint8)
+                self._packs = np.empty(int(npacks.value * 1.25) + 64, dtype=np.uint64)
+                continue
+            self._check(rc)
+            return o[:nbytes.value], pk[:npacks.value], list(frags)
+        raise KmcB200Error(ERR_CAPACITY, "kmcb200_split: buffers still too small")
+
+    def split(self, batch):
+        """One batch -> one SuperKmerBin fragment per bin (copies; empty bins have size 0)."""
+        out, packs, frags = self.split_raw(batch)
+        res = []
+        for f in frags:
+            res.append(SuperKmerBin(data=out[f.byte_off:f.byte_off + f.bytes].copy(), n_rec=int(f.n_rec),
+                                    pack_bytes=packs[f.pack0:f.pack0 + f.n_packs].copy(), n_super_kmers=int(f.n_super_kmers), kmer_len=self.kmer_len))
+        return res
+
+    def dev_split(self, d_seq, nbytes, d_out, out_capacity, d_pack_bytes, pack_capacity, d_frags, d_result, stream=None):
+        """kmcb200_dev_split: device pointers (ints or tensors' data_ptr()); d_frags holds n_bins x 40 bytes, d_result 5 x uint64."""
+        self._check(self.lib.kmcb200_dev_split(self._h, d_seq, nbytes, d_out, out_capacity, d_pack_bytes, pack_capacity, d_frags, d_result, stream))

@@ -12,6 +12,7 @@
 #include "leaf_warp.cuh"
 #include "leaf_hash.cuh"
 #include "leaf_hash_wide.cuh"
+#include "split.cuh"
 
 #include <cmath>
 #include <cstddef>
@@ -1755,3 +1756,4 @@ int kmcb200_stage_names(kmcb200_ctx* ctx, uint32_t slot, char* buf, uint32_t cap
 }  // extern "C"
 
 #include "db_writer.inl"
+#include "splitter.inl"

@@ -208,6 +208,60 @@ int kmcb200_dev_split(kmcb200_splitter* sp, const uint8_t* d_seq, uint64_t bytes
 	uint64_t* d_pack_bytes, uint64_t pack_capacity, kmcb200_bin_fragment* d_frags, uint64_t* d_result, void* stream);
 /* Number of kernels this splitter has launched so far. */
 uint64_t kmcb200_splitter_kernel_launches(const kmcb200_splitter* sp);
+/* Opt-in: from now on every split also adds, per bin, the (k+x)-mer count of its records that CKmerBinCollector keeps in n_plus_x_recs
+ * (kb_collector.cpp:73-89) with max_x = k % 32 ? min(31 - k % 32, 3) : 0 (kmc.h:139-142): 1 + (n - k) / (max_x + 1) per record of n
+ * symbols when both_strands == 0, the collector's strand-state walk (kb_collector.h:66-116) when it is 1; nothing when max_x = 0.  This
+ * is what kmcb200_stage2_bin_order needs.  The call zeroes the totals; a split that ends in KMCB200_ERR_CAPACITY (or a capacity flag on
+ * the device) adds nothing.  One more kernel per split; a splitter that never calls this launches and writes exactly as before. */
+int kmcb200_splitter_count_kxmers(kmcb200_splitter* sp, int both_strands);
+/* per_bin[n_bins]: the totals since kmcb200_splitter_count_kxmers (waits for the device's queued work).  KMCB200_ERR_INVALID when the
+ * counting was never enabled. */
+int kmcb200_splitter_kxmer_totals(kmcb200_splitter* sp, uint64_t* per_bin);
+
+/* ---- stage 0: signature statistics (CKMC::buildSignatureMapping, kmc_core/kmc.h:974-1075) ----------------------------------------
+ * Before it splits, the reference counts the k-mers of every signature over a sample of the input (CSplitter::CalcStats,
+ * splitter.cpp:439-533) and groups the signatures into n_bins bins by those counts (CSignatureMapper::Init, s_mapper.h:141-235).  After
+ * the split, its stage 2 with one thread (-sr1) reads the bins in descending order of their memory need (CBinDesc::get_sorted_req_sizes,
+ * queues.h:499-558), and that order is the bins' order in the database and the value the .kmc_pre map stores for their signatures.
+ *   kmcb200_sigstats_*        the statistics on the GPU; the batch format is kmcb200_split's (every byte other than ACGTacgt separates);
+ *                             counts[sig] += 1 for every k-mer of ACGT only, sig = its least normalised m-mer (4^m: the special signature),
+ *                             accumulated over calls until reset, 32-bit counters that wrap like the reference's.  Workspace: the batch
+ *                             (max_batch_bytes, host path) and the 4^m + 1 counters; nothing per base.
+ *   kmcb200_signature_map     Init on the host: map[sig] = bin id, -1 for a signature that is not allowed (no k-mer ever has it; the
+ *                             completer stores 0 for it).  Needs no device.
+ *   kmcb200_stage2_bin_order  get_sorted_req_sizes + get_req_size on the host: file_pos[bin] = the bin's position in the database.  bytes,
+ *                             n_rec and n_plus_x_recs are per bin over the whole input (kmcb200_bin_fragment's bytes / n_rec summed,
+ *                             kmcb200_splitter_kxmer_totals; n_plus_x_recs may be NULL when k % 32 == 0).  Needs no device.
+ * Host-function failures leave their message in kmcb200_sigstats_last_error(NULL). */
+typedef struct kmcb200_sigstats kmcb200_sigstats;
+typedef struct {
+	uint32_t kmer_len;                    /* signature_len+1 .. KMCB200_MAX_KMER_LEN */
+	uint32_t signature_len;               /* 5..11 */
+	int32_t device;                       /* CUDA ordinal */
+	uint32_t reserved;                    /* 0 */
+	uint64_t max_batch_bytes;             /* largest batch one call accepts (1..KMCB200_SPLIT_MAX_BATCH) */
+} kmcb200_sigstats_params;
+/* KMCB200_ERR_INVALID for a bad parameter, KMCB200_ERR_NO_DEVICE without an sm_90 device (no CPU fallback).  The counters start at 0. */
+int kmcb200_sigstats_create(const kmcb200_sigstats_params* params, kmcb200_sigstats** out);
+void kmcb200_sigstats_destroy(kmcb200_sigstats* h);
+/* message of the last failure on this handle (or of the last failed create / host function when h == NULL) */
+const char* kmcb200_sigstats_last_error(const kmcb200_sigstats* h);
+/* Host batch: copied in, counted; returns when the batch buffer may be reused.  A batch over max_batch_bytes: KMCB200_ERR_INVALID. */
+int kmcb200_sigstats_add(kmcb200_sigstats* h, const uint8_t* seq, uint64_t bytes);
+/* Device twin: d_seq in HBM, queued on `stream` (a cudaStream_t; NULL = the legacy default stream) after the handle's earlier work. */
+int kmcb200_dev_sigstats_add(kmcb200_sigstats* h, const uint8_t* d_seq, uint64_t bytes, void* stream);
+/* counts[4^signature_len + 1] (host) after every call queued so far, device twin included. */
+int kmcb200_sigstats_read(kmcb200_sigstats* h, uint32_t* counts);
+int kmcb200_sigstats_reset(kmcb200_sigstats* h);
+/* Number of kernels this handle has launched so far. */
+uint64_t kmcb200_sigstats_kernel_launches(const kmcb200_sigstats* h);
+/* map[4^signature_len + 1].  KMCB200_ERR_INVALID: signature_len outside 5..11, n_bins outside 2..KMCB200_SPLIT_MAX_BINS (one bin besides
+ * the special signature's is needed), or counts for which the rule would hand out an id >= n_bins. */
+int kmcb200_signature_map(const uint32_t* counts, uint32_t signature_len, uint32_t n_bins, int32_t* map);
+/* file_pos[n_bins]: a permutation of 0..n_bins-1.  cutoff_max / counter_max as the database's parameters; records are 8 * ceil(k / 32) bytes
+ * (sizeof(CKmer<SIZE>)) and every buffer is rounded to 256 bytes (ALIGNMENT), as in the reference. */
+int kmcb200_stage2_bin_order(uint32_t n_bins, const uint64_t* bytes, const uint64_t* n_rec, const uint64_t* n_plus_x_recs, uint32_t kmer_len,
+	uint32_t cutoff_min, uint64_t cutoff_max, uint64_t counter_max, uint32_t lut_prefix_len, uint32_t* file_pos);
 
 /* ---- seam #1: sort host records ------------------------------------------------------------------
  * Contract of SortFunction (raduls.h:19-20, kb_sorter.h:775-779): n records of rec_bytes (multiple of 8,

@@ -39,6 +39,10 @@ class _SplitParams(C.Structure):
     _fields_ = [("kmer_len", C.c_uint32), ("signature_len", C.c_uint32), ("n_bins", C.c_uint32), ("device", C.c_int32), ("max_batch_bytes", C.c_uint64)]
 
 
+class _SigstatsParams(C.Structure):
+    _fields_ = [("kmer_len", C.c_uint32), ("signature_len", C.c_uint32), ("device", C.c_int32), ("reserved", C.c_uint32), ("max_batch_bytes", C.c_uint64)]
+
+
 class BinFragment(C.Structure):
     """kmcb200_bin_fragment: one bin's share of a split batch."""
     _fields_ = [("byte_off", C.c_uint64), ("bytes", C.c_uint64), ("n_rec", C.c_uint64), ("n_super_kmers", C.c_uint64),
@@ -52,7 +56,9 @@ EXPORTS = [
     "kmcb200_stage_times", "kmcb200_stage_names",
     "kmcb200_wait_bin_scanned", "kmcb200_db_open", "kmcb200_db_last_error", "kmcb200_db_records", "kmcb200_db_reserve", "kmcb200_db_commit_bin", "kmcb200_db_close",
     "kmcb200_splitter_create", "kmcb200_splitter_destroy", "kmcb200_splitter_last_error", "kmcb200_split", "kmcb200_dev_split",
-    "kmcb200_splitter_kernel_launches",
+    "kmcb200_splitter_kernel_launches", "kmcb200_splitter_count_kxmers", "kmcb200_splitter_kxmer_totals",
+    "kmcb200_sigstats_create", "kmcb200_sigstats_destroy", "kmcb200_sigstats_last_error", "kmcb200_sigstats_add", "kmcb200_dev_sigstats_add",
+    "kmcb200_sigstats_read", "kmcb200_sigstats_reset", "kmcb200_sigstats_kernel_launches", "kmcb200_signature_map", "kmcb200_stage2_bin_order",
 ]
 
 _lib = None
@@ -114,6 +120,21 @@ def load_library(build_if_needed=True):
     L.kmcb200_dev_split.argtypes = [vp, vp, u64, vp, u64, vp, u64, vp, vp, vp]
     L.kmcb200_splitter_kernel_launches.argtypes = [vp]
     L.kmcb200_splitter_kernel_launches.restype = u64
+    L.kmcb200_splitter_count_kxmers.argtypes = [vp, C.c_int]
+    L.kmcb200_splitter_kxmer_totals.argtypes = [vp, vp]
+    L.kmcb200_sigstats_create.argtypes = [C.POINTER(_SigstatsParams), C.POINTER(vp)]
+    L.kmcb200_sigstats_destroy.argtypes = [vp]
+    L.kmcb200_sigstats_destroy.restype = None
+    L.kmcb200_sigstats_last_error.argtypes = [vp]
+    L.kmcb200_sigstats_last_error.restype = C.c_char_p
+    L.kmcb200_sigstats_add.argtypes = [vp, vp, u64]
+    L.kmcb200_dev_sigstats_add.argtypes = [vp, vp, u64, vp]
+    L.kmcb200_sigstats_read.argtypes = [vp, vp]
+    L.kmcb200_sigstats_reset.argtypes = [vp]
+    L.kmcb200_sigstats_kernel_launches.argtypes = [vp]
+    L.kmcb200_sigstats_kernel_launches.restype = u64
+    L.kmcb200_signature_map.argtypes = [vp, u32, u32, vp]
+    L.kmcb200_stage2_bin_order.argtypes = [u32, vp, vp, vp, u32, u32, u64, u64, u32, vp]
     _lib = L
     return L
 
@@ -400,3 +421,95 @@ class Splitter:
     def dev_split(self, d_seq, nbytes, d_out, out_capacity, d_pack_bytes, pack_capacity, d_frags, d_result, stream=None):
         """kmcb200_dev_split: device pointers (ints or tensors' data_ptr()); d_frags holds n_bins x 40 bytes, d_result 5 x uint64."""
         self._check(self.lib.kmcb200_dev_split(self._h, d_seq, nbytes, d_out, out_capacity, d_pack_bytes, pack_capacity, d_frags, d_result, stream))
+
+    def count_kxmers(self, both_strands=True):
+        """From now on every split also counts, per bin, the collector's (k+x)-mers (n_plus_x_recs); zeroes the totals."""
+        self._check(self.lib.kmcb200_splitter_count_kxmers(self._h, int(bool(both_strands))))
+
+    def kxmer_totals(self):
+        """uint64[n_bins]: the (k+x)-mers per bin since count_kxmers (zeros for k % 32 == 0, where stage 2 sorts plain k-mers)."""
+        out = np.zeros(self.n_bins, dtype=np.uint64)
+        self._check(self.lib.kmcb200_splitter_kxmer_totals(self._h, out.ctypes.data))
+        return out
+
+
+class SignatureStats:
+    """Stage 0 on one GPU (kmcb200_sigstats_*): k-mers per signature over batches of sequences, what CSplitter::CalcStats counts
+    (kmc_core/splitter.cpp:439-533).  Batches as for Splitter; the counts (uint32[4^signature_len + 1]) add up until reset()."""
+
+    def __init__(self, kmer_len, signature_len, device=0, max_batch_bytes=1 << 26):
+        self.lib = load_library()
+        self.kmer_len, self.signature_len, self.max_batch_bytes = kmer_len, signature_len, max_batch_bytes
+        self._h = C.c_void_p(None)
+        p = _SigstatsParams(kmer_len, signature_len, device, 0, max_batch_bytes)
+        rc = self.lib.kmcb200_sigstats_create(C.byref(p), C.byref(self._h))
+        if rc != 0:
+            raise KmcB200Error(rc, (self.lib.kmcb200_sigstats_last_error(None) or b"").decode())
+
+    def _check(self, rc):
+        if rc < 0:
+            raise KmcB200Error(rc, (self.lib.kmcb200_sigstats_last_error(self._h) or b"").decode())
+        return rc
+
+    def close(self):
+        if self._h:
+            self.lib.kmcb200_sigstats_destroy(self._h)
+            self._h = C.c_void_p(None)
+
+    def __del__(self):
+        try:
+            self.close()
+        except Exception:
+            pass
+
+    def kernel_launches(self):
+        return int(self.lib.kmcb200_sigstats_kernel_launches(self._h))
+
+    def add(self, batch):
+        seq = np.ascontiguousarray(np.frombuffer(batch, dtype=np.uint8) if isinstance(batch, (bytes, bytearray)) else batch, dtype=np.uint8)
+        self._check(self.lib.kmcb200_sigstats_add(self._h, seq.ctypes.data, seq.size))
+
+    def dev_add(self, d_seq, nbytes, stream=None):
+        """kmcb200_dev_sigstats_add: d_seq a device pointer (int or a tensor's data_ptr()), queued on `stream` (a cudaStream_t)."""
+        self._check(self.lib.kmcb200_dev_sigstats_add(self._h, d_seq, nbytes, stream))
+
+    def read(self):
+        out = np.zeros((1 << (2 * self.signature_len)) + 1, dtype=np.uint32)
+        self._check(self.lib.kmcb200_sigstats_read(self._h, out.ctypes.data))
+        return out
+
+    def reset(self):
+        self._check(self.lib.kmcb200_sigstats_reset(self._h))
+
+
+def _host_check(lib, rc):
+    if rc < 0:
+        raise KmcB200Error(rc, (lib.kmcb200_sigstats_last_error(None) or b"").decode())
+
+
+def signature_map(counts, signature_len, n_bins):
+    """CSignatureMapper::Init (kmc_core/s_mapper.h:141-235) on the host: int32[4^signature_len + 1] bin ids from per-signature k-mer counts,
+    -1 for the signatures that are not allowed (no k-mer has them).  Needs no GPU."""
+    lib = load_library()
+    cnt = np.ascontiguousarray(counts, dtype=np.uint32)
+    if cnt.size != (1 << (2 * signature_len)) + 1:
+        raise KmcB200Error(ERR_INVALID, "counts has %d entries, 4^%d + 1 expected" % (cnt.size, signature_len))
+    out = np.zeros(cnt.size, dtype=np.int32)
+    _host_check(lib, lib.kmcb200_signature_map(cnt.ctypes.data, signature_len, n_bins, out.ctypes.data))
+    return out
+
+
+def stage2_bin_order(bytes_per_bin, n_rec, n_plus_x_recs, kmer_len, cutoff_min, cutoff_max, counter_max, lut_prefix_len):
+    """The reference's stage-2 order of the bins with one thread (CBinDesc::get_sorted_req_sizes, kmc_core/queues.h:499-558) on the host:
+    uint32[n_bins], every bin's position in the database.  Needs no GPU."""
+    lib = load_library()
+    b = np.ascontiguousarray(bytes_per_bin, dtype=np.uint64)
+    r = np.ascontiguousarray(n_rec, dtype=np.uint64)
+    x = None if n_plus_x_recs is None else np.ascontiguousarray(n_plus_x_recs, dtype=np.uint64)
+    if r.size != b.size or (x is not None and x.size != b.size):
+        raise KmcB200Error(ERR_INVALID, "per-bin arrays of different lengths")
+    out = np.zeros(b.size, dtype=np.uint32)
+    _host_check(lib, lib.kmcb200_stage2_bin_order(b.size, b.ctypes.data, r.ctypes.data, None if x is None else x.ctypes.data, kmer_len, cutoff_min,
+                                                  min(int(cutoff_max), (1 << 64) - 1), min(int(counter_max), (1 << 64) - 1), lut_prefix_len,
+                                                  out.ctypes.data))
+    return out

@@ -23,6 +23,7 @@
 #include <string>
 #include <vector>
 #include <algorithm>
+#include <list>
 #include <thread>
 
 using namespace kmcb;
@@ -1757,3 +1758,4 @@ int kmcb200_stage_names(kmcb200_ctx* ctx, uint32_t slot, char* buf, uint32_t cap
 
 #include "db_writer.inl"
 #include "splitter.inl"
+#include "stage0.inl"

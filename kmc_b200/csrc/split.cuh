@@ -20,6 +20,9 @@
 //   split_frag_kernel        per-bin fragments, pack numbering, sizes and the capacity check
 //   split_pack_bytes_kernel  pack lengths
 //   split_emit_kernel        the packed records, written at their offsets
+//   split_kxmer_kernel       opt-in (kmcb200_splitter_count_kxmers): per record tile, the collector's (k+x)-mer count per bin
+// Stage 0 shares the windowed minimum (split_window_table) and adds one kernel of its own:
+//   sigstats_kernel          k-mers per signature over a batch (CSplitter::CalcStats), runs aggregated per warp before the global atomics
 #pragma once
 #include "common.cuh"
 
@@ -106,21 +109,16 @@ __device__ __forceinline__ uint64_t split_block_excl(uint64_t v, uint64_t* s_war
 }
 
 // ------------------------------------------------------------------------------------------------ per k-mer signatures
-// Tile = kSplitTile k-mer positions t0 .. t0+T-1, plus t0-1 (for the run start at t0).  Loads the bases [t0-1, t0+T+k-1).
-// sig[t] = min of the m-mer values of the k-mer at t, with kSplitInvalid set when the k-mer holds a non-ACGT byte or runs past the batch.
-// tile_last[tile] = 1 + the last position of the tile where a run of equal signatures starts (0: none).
-__global__ void __launch_bounds__(kSplitThreads) split_signature_kernel(const uint8_t* __restrict__ seq, uint64_t len, uint32_t k, uint32_t m,
-	uint32_t* __restrict__ sig, uint64_t* __restrict__ tile_last)
+// The windowed minimum of one tile (kSplitTile k-mer positions t0 .. t0+T-1, plus t0-1): loads the bases [t0-1, t0+T+k-1) into s_code,
+// their normalised m-mer values into s_val, and folds s_val into a log-step sparse table.  Returns `span`: the signature of position
+// t0-1+i is then split_window_sig(s_val, i, w, span).  Called by every thread of the CTA; ends with a barrier.
+__device__ __forceinline__ uint32_t split_window_table(const uint8_t* __restrict__ seq, uint64_t len, uint64_t t0, uint32_t k, uint32_t m,
+	uint8_t* s_code /* [kSplitTile + kSplitMaxSpan + 8] */, uint32_t* s_val /* [kSplitTile + kSplitMaxSpan + 8] */)
 {
-	__shared__ uint8_t s_code[kSplitTile + kSplitMaxSpan + 8];
-	__shared__ uint32_t s_val[kSplitTile + kSplitMaxSpan + 8];
-	__shared__ uint32_t s_last;
 	constexpr uint32_t kPer = (kSplitTile + kSplitMaxSpan + kSplitThreads) / kSplitThreads;
 	const uint32_t tid = threadIdx.x;
-	const uint64_t t0 = (uint64_t)blockIdx.x * kSplitTile;
 	const uint32_t w = k - m + 1;
 	const uint32_t n_base = kSplitTile + k, n_val = kSplitTile + w;
-	if (tid == 0) s_last = 0;
 	for (uint32_t i = tid; i < n_base; i += kSplitThreads) {
 		const int64_t b = (int64_t)t0 - 1 + (int64_t)i;
 		s_code[i] = (b >= 0 && (uint64_t)b < len) ? (uint8_t)split_code(seq[b]) : (uint8_t)4;
@@ -155,13 +153,35 @@ __global__ void __launch_bounds__(kSplitThreads) split_signature_kernel(const ui
 		__syncthreads();
 		span *= 2;
 	}
+	return span;
+}
+
+// signature word of position t0-1+i of a tile after split_window_table (w = k - m + 1 m-mers per k-mer)
+__device__ __forceinline__ uint32_t split_window_sig(const uint32_t* s_val, uint32_t i, uint32_t w, uint32_t span)
+{
+	return split_combine(s_val[i], s_val[i + w - span]);
+}
+
+// sig[t] = min of the m-mer values of the k-mer at t, with kSplitInvalid set when the k-mer holds a non-ACGT byte or runs past the batch.
+// tile_last[tile] = 1 + the last position of the tile where a run of equal signatures starts (0: none).
+__global__ void __launch_bounds__(kSplitThreads) split_signature_kernel(const uint8_t* __restrict__ seq, uint64_t len, uint32_t k, uint32_t m,
+	uint32_t* __restrict__ sig, uint64_t* __restrict__ tile_last)
+{
+	__shared__ uint8_t s_code[kSplitTile + kSplitMaxSpan + 8];
+	__shared__ uint32_t s_val[kSplitTile + kSplitMaxSpan + 8];
+	__shared__ uint32_t s_last;
+	const uint32_t tid = threadIdx.x;
+	const uint64_t t0 = (uint64_t)blockIdx.x * kSplitTile;
+	const uint32_t w = k - m + 1;
+	if (tid == 0) s_last = 0;
+	const uint32_t span = split_window_table(seq, len, t0, k, m, s_code, s_val);
 	// positions t0-1+i for i = tid*16 .. tid*16+16
 	const uint32_t i0 = tid * kSplitPerThread;
-	uint32_t prev = split_combine(s_val[i0], s_val[i0 + w - span]);
+	uint32_t prev = split_window_sig(s_val, i0, w, span);
 	uint32_t last = 0;
 	for (uint32_t e = 1; e <= kSplitPerThread; ++e) {
 		const uint32_t i = i0 + e;
-		const uint32_t cur = split_combine(s_val[i], s_val[i + w - span]);
+		const uint32_t cur = split_window_sig(s_val, i, w, span);
 		const uint64_t t = t0 - 1 + i;
 		if (t < len) {
 			sig[t] = cur;
@@ -172,6 +192,65 @@ __global__ void __launch_bounds__(kSplitThreads) split_signature_kernel(const ui
 	if (last) atomicMax(&s_last, last);
 	__syncthreads();
 	if (tid == 0) tile_last[blockIdx.x] = s_last;
+}
+
+// ------------------------------------------------------------------------------------------------ stage 0: k-mers per signature
+// counts[sig] += the valid k-mers of the tile whose signature is sig (CSplitter::CalcStats, kmc_core/splitter.cpp:439-533, adds up the same
+// numbers read by read).  Same tiles and windowed minimum as split_signature_kernel, but nothing per position leaves the chip: a run of equal
+// signatures is counted where it ends.  Thread j of a warp holds 16 consecutive positions; the length of a run that enters it from lane
+// j-1 (carry) comes from a segmented scan over the lanes, so a run costs one global atomic per warp it touches, however long it is.
+__global__ void __launch_bounds__(kSplitThreads) sigstats_kernel(const uint8_t* __restrict__ seq, uint64_t len, uint32_t k, uint32_t m,
+	uint32_t* __restrict__ counts)
+{
+	__shared__ uint8_t s_code[kSplitTile + kSplitMaxSpan + 8];
+	__shared__ uint32_t s_val[kSplitTile + kSplitMaxSpan + 8];
+	const uint32_t tid = threadIdx.x, lane = tid & 31u;
+	const uint64_t t0 = (uint64_t)blockIdx.x * kSplitTile;
+	const uint32_t w = k - m + 1;
+	const uint32_t span = split_window_table(seq, len, t0, k, m, s_code, s_val);
+	// this thread's positions t0 + 16 tid + e, e = 0..15, and the one before them
+	const uint32_t i0 = tid * kSplitPerThread;
+	const uint32_t before = split_window_sig(s_val, i0, w, span);
+	uint32_t s[kSplitPerThread];
+#pragma unroll
+	for (uint32_t e = 0; e < kSplitPerThread; ++e) s[e] = split_window_sig(s_val, i0 + 1 + e, w, span);
+	// in: position 0 continues the run of the position before it (lane 0 starts the warp's runs afresh)
+	const bool in = lane != 0 && !(s[0] & kSplitInvalid) && s[0] == before;
+	// tail: length of the run that ends at position 15 (0 when position 15 is invalid); whole: one run covers all 16 positions
+	uint32_t tail = (s[kSplitPerThread - 1] & kSplitInvalid) ? 0u : 1u;
+	bool open = tail != 0;
+#pragma unroll
+	for (int e = (int)kSplitPerThread - 2; e >= 0; --e) {
+		open = open && s[e] == s[e + 1];
+		tail += open;
+	}
+	const bool whole = tail == kSplitPerThread;
+	// carry_j = in_j ? tail_{j-1} + (whole_{j-1} ? carry_{j-1} : 0) : 0, as an inclusive scan of the affine maps c -> a + b c
+	const uint32_t prev_tail = __shfl_up_sync(0xffffffffu, tail, 1);
+	const bool prev_whole = __shfl_up_sync(0xffffffffu, (uint32_t)whole, 1) != 0;
+	uint32_t a = in ? prev_tail : 0u, b = (in && prev_whole) ? 1u : 0u;
+#pragma unroll
+	for (uint32_t o = 1; o < 32; o <<= 1) {
+		const uint32_t pa = __shfl_up_sync(0xffffffffu, a, o), pb = __shfl_up_sync(0xffffffffu, b, o);
+		if (lane >= o) { a += b * pa; b *= pb; }
+	}
+	const uint32_t carry = a;
+	// out: the run that ends at position 15 goes on into lane j+1, which counts it
+	const bool out = __shfl_down_sync(0xffffffffu, (uint32_t)in, 1) != 0 && lane != 31;
+	uint32_t run = 0;
+	bool first = true;                                                  // the current run started at position 0
+#pragma unroll
+	for (uint32_t e = 0; e < kSplitPerThread; ++e) {
+		const uint32_t v = s[e];
+		if (v & kSplitInvalid) { first = false; continue; }
+		++run;
+		const bool ends = e + 1 == kSplitPerThread ? !out : s[e + 1] != v;
+		if (ends) {
+			atomicAdd(&counts[v], run + (first && in ? carry : 0u));
+			run = 0;
+			first = false;
+		}
+	}
 }
 
 // ------------------------------------------------------------------------------------------------ device scans (in place, exclusive)
@@ -329,6 +408,60 @@ __global__ void __launch_bounds__(kSplitThreads) split_bin_hist_kernel(const uin
 			atomicAdd(&bin_recs[b], (unsigned long long)s_hist[2 * n_bins + b]);
 		}
 	}
+}
+
+// ------------------------------------------------------------------------------------------------ (k+x)-mers per bin (opt-in)
+// The collector's n_plus_x_recs of one canonical record of n symbols (CKmerBinCollector::update_n_plus_x_recs, kb_collector.h:66-116):
+// along the record, the order of the last 4 symbols of the k-mer and of its reverse complement's first 4 gives a state; a stretch of one
+// strict state of x + 1 k-mers counts 1 + x / div, every k-mer of the equal state counts 1.
+__device__ __forceinline__ uint32_t split_kxmer_canonical(const uint8_t* __restrict__ p, uint32_t n, uint32_t k, uint32_t div)
+{
+	auto sym = [&](uint32_t i) { return split_code(p[i]) & 3u; };
+	auto order = [](uint32_t f, uint32_t r) { return f < r ? 0u : (r < f ? 1u : 2u); };
+	uint32_t fw = (sym(0) << 6) | (sym(1) << 4) | (sym(2) << 2) | sym(3);
+	uint32_t rc = ((3u - sym(k - 1)) << 6) | ((3u - sym(k - 2)) << 4) | ((3u - sym(k - 3)) << 2) | (3u - sym(k - 4));
+	uint32_t cur = order(fw, rc), x = 0, total = 0;
+	for (uint32_t i = 0; i + k < n; ++i) {
+		rc = (rc >> 2) | ((3u - sym(k + i)) << 6);
+		fw = ((fw << 2) | sym(4 + i)) & 0xffu;
+		const uint32_t st = order(fw, rc);
+		if (st == cur) {
+			if (cur == 2) ++total;
+			else ++x;
+		} else {
+			cur = st;
+			total += 1 + x / div;
+			x = 0;
+		}
+	}
+	return total + 1 + x / div;
+}
+
+// Same record tiles as split_bin_hist_kernel (after it: rec_bin is set).  kx[b] += the (k+x)-mers of bin b's records, max_x > 0:
+// 1 + (n - k) / (max_x + 1) per record of n symbols for plain k-mers (kb_collector.cpp:76-78), split_kxmer_canonical for canonical ones.
+// Nothing is added for a batch whose outputs do not fit (the split writes nothing then either).
+__global__ void __launch_bounds__(kSplitThreads) split_kxmer_kernel(const uint8_t* __restrict__ seq, const uint32_t* __restrict__ rec_start,
+	const uint32_t* __restrict__ rec_end, const uint32_t* __restrict__ rec_bin, uint32_t k, uint32_t max_x, uint32_t both_strands, uint32_t n_bins,
+	const uint64_t* __restrict__ state, unsigned long long* __restrict__ kx)
+{
+	extern __shared__ uint32_t s_kx[];                                 // [n_bins]
+	if (state[kStCapErr]) return;
+	const uint64_t n_rec = state[kStRecords];
+	const uint64_t n_rt = (n_rec + kSplitRecTile - 1) / kSplitRecTile;
+	if (blockIdx.x >= n_rt) return;
+	for (uint32_t b = threadIdx.x; b < n_bins; b += blockDim.x) s_kx[b] = 0;
+	__syncthreads();
+	const uint64_t r0 = (uint64_t)blockIdx.x * kSplitRecTile;
+	const uint64_t r1 = r0 + kSplitRecTile < n_rec ? r0 + kSplitRecTile : n_rec;
+	for (uint64_t r = r0 + threadIdx.x; r < r1; r += blockDim.x) {
+		const uint32_t s = rec_start[r];
+		const uint32_t n = rec_end[r] - s + k;
+		const uint32_t v = both_strands ? split_kxmer_canonical(seq + s, n, k, max_x + 1) : 1u + (n - k) / (max_x + 1);
+		atomicAdd(&s_kx[rec_bin[r]], v);
+	}
+	__syncthreads();
+	for (uint32_t b = threadIdx.x; b < n_bins; b += blockDim.x)
+		if (s_kx[b]) atomicAdd(&kx[b], (unsigned long long)s_kx[b]);
 }
 
 __device__ __forceinline__ uint64_t split_bin_base(const uint64_t* hist, uint64_t n_rt, uint32_t b, uint32_t n_bins, const uint64_t* state)

@@ -196,7 +196,8 @@ void kmcb200_splitter_destroy(kmcb200_splitter* sp);
 /* message of the last failure on this splitter (or of the last failed kmcb200_splitter_create when sp == NULL) */
 const char* kmcb200_splitter_last_error(const kmcb200_splitter* sp);
 /* Host buffers: copies the batch in and returns when out[0, *out_bytes), pack_bytes[0, *n_packs) and frags[n_bins] are filled.  When
- * out_capacity or pack_capacity is too small: KMCB200_ERR_CAPACITY, *out_bytes / *n_packs give the required sizes, nothing else is written. */
+ * out_capacity or pack_capacity is too small: KMCB200_ERR_CAPACITY, *out_bytes / *n_packs give the required sizes, nothing else is written.
+ * For raw FASTQ / FASTA bytes instead of a batch, see kmcb200_split_fastx ("reads text -> batch" below). */
 int kmcb200_split(kmcb200_splitter* sp, const uint8_t* seq, uint64_t bytes,
 	uint8_t* out, uint64_t out_capacity, uint64_t* out_bytes,
 	uint64_t* pack_bytes, uint64_t pack_capacity, uint64_t* n_packs, kmcb200_bin_fragment* frags);
@@ -262,6 +263,58 @@ int kmcb200_signature_map(const uint32_t* counts, uint32_t signature_len, uint32
  * (sizeof(CKmer<SIZE>)) and every buffer is rounded to 256 bytes (ALIGNMENT), as in the reference. */
 int kmcb200_stage2_bin_order(uint32_t n_bins, const uint64_t* bytes, const uint64_t* n_rec, const uint64_t* n_plus_x_recs, uint32_t kmer_len,
 	uint32_t cutoff_min, uint64_t cutoff_max, uint64_t counter_max, uint32_t lut_prefix_len, uint32_t* file_pos);
+
+/* ---- reads text -> batch: FASTQ / FASTA parsed on the GPU ------------------------------------------------------------------------
+ * kmcb200_split and kmcb200_sigstats_add take batches in which every non-ACGT byte separates; raw FASTQ cannot be passed as it is (quality
+ * lines hold A, C, G, T), nor FASTA (headers hold letters).  This parser makes that batch from raw file bytes on the GPU, one chunk at a
+ * time, byte for byte what kmc_b200.reads.sequences_to_batch makes of the whole file (the chunks' outputs, concatenated):
+ *   FASTQ  line 1 of every 4 is kept with its '\n'; lines are counted from the chunk's start, so every chunk must start on a record;
+ *   FASTA  a header line (first byte '>') becomes one '\n', every other line is kept without its '\n', blank lines vanish.
+ * '\r' is an ordinary byte (a separator in the batch).  A final chunk that does not end in '\n' is parsed as if it did, so the output
+ * never exceeds bytes + 1.  The format is the caller's choice (the file's first non-empty line starts with '@' or '>'); gzip is not read.
+ * Records end after every 4th line (FASTQ) or where a header line starts after a '\n' (FASTA); the end of a final chunk ends one too.
+ *   is_final == 0  the chunk is parsed up to its last record end, returned as `consumed`: the caller carries the rest into the next chunk.
+ *                  A chunk without a record end is KMCB200_ERR_INVALID ("a record is longer than the chunk") and nothing else is written.
+ *   limit < bytes  only the records that start before `limit` are parsed: the cut is the first record end at or past `limit` (where the
+ *                  chunk has one; a non-final chunk without one is parsed to its last record end, so consumed < limit says "go on").
+ *                  KMCB200_FASTX_NO_LIMIT (or any limit >= bytes): no cut.
+ * Work per call: 9 kernel launches whatever the size, no host synchronisation inside (consumed, the cut and the error are decided on the
+ * device).  Workspace: the chunk and the output of the host-buffer form (2 B per byte of max_chunk_bytes) plus 120 B per 16 KiB tile. */
+#define KMCB200_FASTQ 1
+#define KMCB200_FASTA 2
+#define KMCB200_FASTX_NO_LIMIT (~0ull)
+typedef struct kmcb200_fastx kmcb200_fastx;
+typedef struct {
+	int32_t device;                       /* CUDA ordinal */
+	uint32_t format;                      /* KMCB200_FASTQ or KMCB200_FASTA */
+	uint64_t max_chunk_bytes;             /* largest chunk one call accepts (1..KMCB200_SPLIT_MAX_BATCH): sizes the workspace */
+} kmcb200_fastx_params;
+/* KMCB200_ERR_INVALID for a bad parameter, KMCB200_ERR_NO_DEVICE without an sm_90 device (no CPU fallback). */
+int kmcb200_fastx_create(const kmcb200_fastx_params* params, kmcb200_fastx** out);
+void kmcb200_fastx_destroy(kmcb200_fastx* p);
+/* message of the last failure on this parser (or of the last failed create when p == NULL) */
+const char* kmcb200_fastx_last_error(const kmcb200_fastx* p);
+/* Number of kernels this parser has launched so far (the _fastx entry points below count theirs here too). */
+uint64_t kmcb200_fastx_kernel_launches(const kmcb200_fastx* p);
+/* Host buffers: copies the chunk in, returns when seq[0, *seq_bytes) holds the batch and *consumed the bytes parsed.  When the batch is
+ * longer than seq_capacity: KMCB200_ERR_CAPACITY, *consumed / *seq_bytes are set and seq is not written. */
+int kmcb200_fastx_parse(kmcb200_fastx* p, const uint8_t* raw, uint64_t bytes, int is_final, uint64_t limit,
+	uint8_t* seq, uint64_t seq_capacity, uint64_t* consumed, uint64_t* seq_bytes);
+/* Device twin: d_raw / d_seq / d_result in HBM, queued on `stream` (a cudaStream_t; NULL = the legacy default stream).  seq_capacity
+ * must be at least bytes + 1 (KMCB200_ERR_INVALID otherwise).  d_result receives 4 x uint64: [0] consumed, [1] sequence bytes, [2] records
+ * parsed, [3] 1 when a non-final chunk has no record end (then [0..2] are 0 and d_seq is not written). */
+int kmcb200_dev_fastx_parse(kmcb200_fastx* p, const uint8_t* d_raw, uint64_t bytes, int is_final, uint64_t limit,
+	uint8_t* d_seq, uint64_t seq_capacity, uint64_t* d_result, void* stream);
+/* kmcb200_split of a raw chunk: copies it in and parses it straight into the splitter's batch buffer, then continues exactly like
+ * kmcb200_split from the size phase on (same outputs, same capacity rule).  *consumed as for kmcb200_fastx_parse; *seq_bytes (may be
+ * NULL) the batch's length.  bytes + 1 > max_batch_bytes: KMCB200_ERR_INVALID.  Errors are reported on the splitter. */
+int kmcb200_split_fastx(kmcb200_splitter* sp, kmcb200_fastx* p, const uint8_t* raw, uint64_t bytes, int is_final,
+	uint8_t* out, uint64_t out_capacity, uint64_t* out_bytes, uint64_t* pack_bytes, uint64_t pack_capacity, uint64_t* n_packs,
+	kmcb200_bin_fragment* frags, uint64_t* consumed, uint64_t* seq_bytes);
+/* kmcb200_sigstats_add of a raw chunk, the same way, with the parse's limit (the statistics' sample ends on a record).  bytes + 1 >
+ * max_batch_bytes: KMCB200_ERR_INVALID.  Errors are reported on the statistics handle. */
+int kmcb200_sigstats_add_fastx(kmcb200_sigstats* h, kmcb200_fastx* p, const uint8_t* raw, uint64_t bytes, int is_final, uint64_t limit,
+	uint64_t* consumed);
 
 /* ---- seam #1: sort host records ------------------------------------------------------------------
  * Contract of SortFunction (raduls.h:19-20, kb_sorter.h:775-779): n records of rec_bytes (multiple of 8,

@@ -43,6 +43,10 @@ class _SigstatsParams(C.Structure):
     _fields_ = [("kmer_len", C.c_uint32), ("signature_len", C.c_uint32), ("device", C.c_int32), ("reserved", C.c_uint32), ("max_batch_bytes", C.c_uint64)]
 
 
+class _FastxParams(C.Structure):
+    _fields_ = [("device", C.c_int32), ("format", C.c_uint32), ("max_chunk_bytes", C.c_uint64)]
+
+
 class BinFragment(C.Structure):
     """kmcb200_bin_fragment: one bin's share of a split batch."""
     _fields_ = [("byte_off", C.c_uint64), ("bytes", C.c_uint64), ("n_rec", C.c_uint64), ("n_super_kmers", C.c_uint64),
@@ -59,7 +63,12 @@ EXPORTS = [
     "kmcb200_splitter_kernel_launches", "kmcb200_splitter_count_kxmers", "kmcb200_splitter_kxmer_totals",
     "kmcb200_sigstats_create", "kmcb200_sigstats_destroy", "kmcb200_sigstats_last_error", "kmcb200_sigstats_add", "kmcb200_dev_sigstats_add",
     "kmcb200_sigstats_read", "kmcb200_sigstats_reset", "kmcb200_sigstats_kernel_launches", "kmcb200_signature_map", "kmcb200_stage2_bin_order",
+    "kmcb200_fastx_create", "kmcb200_fastx_destroy", "kmcb200_fastx_last_error", "kmcb200_fastx_kernel_launches", "kmcb200_fastx_parse",
+    "kmcb200_dev_fastx_parse", "kmcb200_split_fastx", "kmcb200_sigstats_add_fastx",
 ]
+
+FASTQ, FASTA = 1, 2                                                     # KMCB200_FASTQ / KMCB200_FASTA
+FASTX_NO_LIMIT = (1 << 64) - 1
 
 _lib = None
 
@@ -135,6 +144,17 @@ def load_library(build_if_needed=True):
     L.kmcb200_sigstats_kernel_launches.restype = u64
     L.kmcb200_signature_map.argtypes = [vp, u32, u32, vp]
     L.kmcb200_stage2_bin_order.argtypes = [u32, vp, vp, vp, u32, u32, u64, u64, u32, vp]
+    L.kmcb200_fastx_create.argtypes = [C.POINTER(_FastxParams), C.POINTER(vp)]
+    L.kmcb200_fastx_destroy.argtypes = [vp]
+    L.kmcb200_fastx_destroy.restype = None
+    L.kmcb200_fastx_last_error.argtypes = [vp]
+    L.kmcb200_fastx_last_error.restype = C.c_char_p
+    L.kmcb200_fastx_kernel_launches.argtypes = [vp]
+    L.kmcb200_fastx_kernel_launches.restype = u64
+    L.kmcb200_fastx_parse.argtypes = [vp, vp, u64, C.c_int, u64, vp, u64, C.POINTER(u64), C.POINTER(u64)]
+    L.kmcb200_dev_fastx_parse.argtypes = [vp, vp, u64, C.c_int, u64, vp, u64, vp, vp]
+    L.kmcb200_split_fastx.argtypes = [vp, vp, vp, u64, C.c_int, vp, u64, C.POINTER(u64), vp, u64, C.POINTER(u64), vp, C.POINTER(u64), C.POINTER(u64)]
+    L.kmcb200_sigstats_add_fastx.argtypes = [vp, vp, vp, u64, C.c_int, u64, C.POINTER(u64)]
     _lib = L
     return L
 
@@ -422,6 +442,25 @@ class Splitter:
         """kmcb200_dev_split: device pointers (ints or tensors' data_ptr()); d_frags holds n_bins x 40 bytes, d_result 5 x uint64."""
         self._check(self.lib.kmcb200_dev_split(self._h, d_seq, nbytes, d_out, out_capacity, d_pack_bytes, pack_capacity, d_frags, d_result, stream))
 
+    def split_fastx(self, parser, raw, is_final=True):
+        """kmcb200_split_fastx: a raw FASTQ / FASTA chunk (bytes or a uint8 array, ideally pinned) parsed on the GPU by `parser` straight into
+        this splitter's batch buffer, then split like split_raw.  Returns (out[:bytes], pack_bytes[:n_packs], fragments, consumed, seq_bytes):
+        a non-final chunk is parsed up to its last record end, and the caller carries raw[consumed:] into the next chunk."""
+        a = _as_u8(raw)
+        frags = (BinFragment * self.n_bins)()
+        nbytes, npacks, consumed, seq_bytes = C.c_uint64(0), C.c_uint64(0), C.c_uint64(0), C.c_uint64(0)
+        for _ in range(2):
+            rc = self.lib.kmcb200_split_fastx(self._h, parser._h, a.ctypes.data, a.size, int(bool(is_final)), self._out.ctypes.data, self._out.size,
+                                              C.byref(nbytes), self._packs.ctypes.data, self._packs.size, C.byref(npacks), frags, C.byref(consumed),
+                                              C.byref(seq_bytes))
+            if rc == ERR_CAPACITY:
+                self._out = np.empty(int(nbytes.value * 1.25) + 1024, dtype=np.uint8)
+                self._packs = np.empty(int(npacks.value * 1.25) + 64, dtype=np.uint64)
+                continue
+            self._check(rc)
+            return self._out[:nbytes.value], self._packs[:npacks.value], list(frags), int(consumed.value), int(seq_bytes.value)
+        raise KmcB200Error(ERR_CAPACITY, "kmcb200_split_fastx: buffers still too small")
+
     def count_kxmers(self, both_strands=True):
         """From now on every split also counts, per bin, the collector's (k+x)-mers (n_plus_x_recs); zeroes the totals."""
         self._check(self.lib.kmcb200_splitter_count_kxmers(self._h, int(bool(both_strands))))
@@ -473,6 +512,15 @@ class SignatureStats:
         """kmcb200_dev_sigstats_add: d_seq a device pointer (int or a tensor's data_ptr()), queued on `stream` (a cudaStream_t)."""
         self._check(self.lib.kmcb200_dev_sigstats_add(self._h, d_seq, nbytes, stream))
 
+    def add_fastx(self, parser, raw, is_final=True, limit=None):
+        """kmcb200_sigstats_add_fastx: a raw FASTQ / FASTA chunk parsed on the GPU by `parser` and counted.  With `limit`, only the records that
+        start before raw[limit] are parsed.  Returns `consumed`, the bytes parsed (the caller carries the rest into its next chunk)."""
+        a = _as_u8(raw)
+        consumed = C.c_uint64(0)
+        self._check(self.lib.kmcb200_sigstats_add_fastx(self._h, parser._h, a.ctypes.data, a.size, int(bool(is_final)),
+                                                        FASTX_NO_LIMIT if limit is None else int(limit), C.byref(consumed)))
+        return int(consumed.value)
+
     def read(self):
         out = np.zeros((1 << (2 * self.signature_len)) + 1, dtype=np.uint32)
         self._check(self.lib.kmcb200_sigstats_read(self._h, out.ctypes.data))
@@ -480,6 +528,66 @@ class SignatureStats:
 
     def reset(self):
         self._check(self.lib.kmcb200_sigstats_reset(self._h))
+
+
+def _as_u8(raw):
+    return np.ascontiguousarray(np.frombuffer(raw, dtype=np.uint8) if isinstance(raw, (bytes, bytearray, memoryview)) else raw, dtype=np.uint8)
+
+
+class FastxParser:
+    """Reads text -> batch on one GPU (kmcb200_fastx_*): raw FASTQ or FASTA chunks become the batches Splitter and SignatureStats take,
+    byte for byte what kmc_b200.reads.sequences_to_batch makes of the whole file.  `fmt` is FASTQ / FASTA (or "fastq" / "fasta"): the
+    caller's choice, by the first byte of the file's first non-empty line.
+
+    A chunk is parsed up to its last record end unless it is final (then to its end, as if it ended in '\n'); `consumed` says where the
+    next chunk must start.  A record longer than the chunk is an error: since the limit here is raw bytes per chunk, a FASTQ record of more
+    than about max_chunk_bytes / 2 bases cannot be parsed, where the host path (sequences_to_batch + batches) accepts sequences up to the
+    batch size."""
+
+    def __init__(self, fmt, device=0, max_chunk_bytes=1 << 26):
+        self.lib = load_library()
+        self.format = {"fastq": FASTQ, "fasta": FASTA}.get(fmt, fmt) if isinstance(fmt, str) else int(fmt)
+        self.max_chunk_bytes = max_chunk_bytes
+        self._h = C.c_void_p(None)
+        p = _FastxParams(device, self.format, max_chunk_bytes)
+        rc = self.lib.kmcb200_fastx_create(C.byref(p), C.byref(self._h))
+        if rc != 0:
+            raise KmcB200Error(rc, (self.lib.kmcb200_fastx_last_error(None) or b"").decode())
+
+    def _check(self, rc):
+        if rc < 0:
+            raise KmcB200Error(rc, (self.lib.kmcb200_fastx_last_error(self._h) or b"").decode())
+        return rc
+
+    def close(self):
+        if self._h:
+            self.lib.kmcb200_fastx_destroy(self._h)
+            self._h = C.c_void_p(None)
+
+    def __del__(self):
+        try:
+            self.close()
+        except Exception:
+            pass
+
+    def kernel_launches(self):
+        return int(self.lib.kmcb200_fastx_kernel_launches(self._h))
+
+    def parse(self, raw, is_final=True, limit=None, out=None):
+        """kmcb200_fastx_parse: (batch, consumed).  `out` (uint8, default: bytes + 1 fresh bytes) receives the batch; a shorter one than the
+        batch raises ERR_CAPACITY and is left untouched."""
+        a = _as_u8(raw)
+        o = np.empty(a.size + 1, dtype=np.uint8) if out is None else out
+        consumed, nbytes = C.c_uint64(0), C.c_uint64(0)
+        self._check(self.lib.kmcb200_fastx_parse(self._h, a.ctypes.data, a.size, int(bool(is_final)), FASTX_NO_LIMIT if limit is None else int(limit),
+                                                 o.ctypes.data, o.size, C.byref(consumed), C.byref(nbytes)))
+        return o[:nbytes.value], int(consumed.value)
+
+    def dev_parse(self, d_raw, nbytes, is_final, limit, d_seq, seq_capacity, d_result, stream=None):
+        """kmcb200_dev_fastx_parse: device pointers (ints or tensors' data_ptr()); seq_capacity >= nbytes + 1; d_result receives 4 x uint64:
+        consumed, sequence bytes, records, error flag (a non-final chunk without a record end)."""
+        self._check(self.lib.kmcb200_dev_fastx_parse(self._h, d_raw, nbytes, int(bool(is_final)), FASTX_NO_LIMIT if limit is None else int(limit),
+                                                     d_seq, seq_capacity, d_result, stream))
 
 
 def _host_check(lib, rc):

@@ -13,6 +13,7 @@
 #include "leaf_hash.cuh"
 #include "leaf_hash_wide.cuh"
 #include "split.cuh"
+#include "fastx.cuh"
 
 #include <cmath>
 #include <cstddef>
@@ -1759,3 +1760,4 @@ int kmcb200_stage_names(kmcb200_ctx* ctx, uint32_t slot, char* buf, uint32_t cap
 #include "db_writer.inl"
 #include "splitter.inl"
 #include "stage0.inl"
+#include "fastx.inl"

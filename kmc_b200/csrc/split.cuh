@@ -322,6 +322,19 @@ __global__ void __launch_bounds__(kSplitThreads) split_scan_down_kernel(uint64_t
 	}
 }
 
+// The three launches of an in-place exclusive scan of a device array (OP 0 = sum, 1 = max) on `st`, with d_partial holding at least
+// ceil(n_max / kSplitScanBlock) words; see split_scan_count for d_cnt / div / mul.  Used by the splitter and the reads-text parser.
+template <int OP>
+inline cudaError_t split_scan_launch(uint64_t* a, uint64_t n_max, const uint64_t* d_cnt, uint64_t div, uint64_t mul, uint64_t* d_total,
+	uint64_t* d_partial, cudaStream_t st)
+{
+	const uint64_t n_blocks = (n_max + kSplitScanBlock - 1) / kSplitScanBlock > 1 ? (n_max + kSplitScanBlock - 1) / kSplitScanBlock : 1;
+	split_scan_reduce_kernel<OP><<<(unsigned)n_blocks, kSplitThreads, 0, st>>>(a, d_cnt, div, mul, n_max, d_partial);
+	split_scan_top_kernel<OP><<<1, kSplitThreads, 0, st>>>(d_partial, n_blocks, d_total);
+	split_scan_down_kernel<OP><<<(unsigned)n_blocks, kSplitThreads, 0, st>>>(a, d_cnt, div, mul, n_max, d_partial);
+	return cudaGetLastError();
+}
+
 // ------------------------------------------------------------------------------------------------ records
 // Same tiles as split_signature_kernel.  carry[tile] = 1 + the last run start before the tile (exclusive max-scan of tile_last).
 // A valid k-mer t starts a record when (t - start of its run) % 256 == 0; it ends one when t+1 is invalid or starts a record.

@@ -15,17 +15,25 @@ its map can differ slightly: the k-mers and their counts are the same, the bins 
 With a map (4^p + 1 entries; `signature_map_from_kmc_pre` reads the one a KMC database was built with) the bins are written in bin-id
 order, and for the same map and parameters the files are byte-identical to the reference CLI's: the bins hold the same k-mers, and stage 2
 and the writer reproduce the reference's output per bin.
+
+Parsing: by default (parse="host") every file is read whole and parsed in numpy (sequences_to_batch).  With parse="gpu" (`--gpu-parse`)
+files are read in chunks of at most batch_bytes - 1 bytes into pinned host buffers by a reader thread, while the GPU parses
+(kmc_b200.FastxParser) and splits the previous chunk; the databases, totals and counts are the same.  A FASTQ / FASTA record must then fit
+in about half a chunk of raw bytes (the rest of a chunk after its last record end is carried into the next one).
 """
 import argparse
 import json
+import os
+import queue
 import struct
 import sys
+import threading
 import time
 
 import numpy as np
 
-from . import DbWriter, KmcB200Error, ERR_INVALID, SignatureStats, Splitter, Stage2Context, Stage2Params, signature_map as _signature_map, \
-    stage2_bin_order
+from . import DbWriter, FASTA, FASTQ, FastxParser, KmcB200Error, ERR_INVALID, SignatureStats, Splitter, Stage2Context, Stage2Params, \
+    signature_map as _signature_map, stage2_bin_order
 
 _NL, _GT, _AT = 10, ord(">"), ord("@")
 STATS_SAMPLE_BYTES = 1 << 28                                            # STATS_FASTQ_SIZE (kmc_core/defs.h)
@@ -70,7 +78,7 @@ def batches(seq, batch_bytes):
         if end >= seq.size:
             yield seq[pos:]
             return
-        i = int(np.searchsorted(seps, end, side="right")) - 1
+        i = int(np.searchsorted(seps, end - 1, side="right")) - 1      # the last separator that keeps the piece within batch_bytes
         if i < 0 or seps[i] < pos:
             raise KmcB200Error(ERR_INVALID, "a sequence is longer than batch_bytes = %d" % batch_bytes)
         yield seq[pos:int(seps[i]) + 1]
@@ -99,12 +107,151 @@ def _record_end(data, at):
     return int(rec_ends[i]) if i < rec_ends.size else a.size
 
 
-def signature_sample_counts(paths, k, signature_len, batch_bytes=1 << 26, device=0):
+def fastx_format(data):
+    """FASTQ or FASTA (kmc_b200.FASTQ / FASTA) by the first byte of the first non-empty line, as sequences_to_batch decides."""
+    a = np.frombuffer(data, dtype=np.uint8) if isinstance(data, (bytes, bytearray, memoryview)) else np.asarray(data, dtype=np.uint8)
+    text = np.flatnonzero(a != _NL)
+    first = int(a[text[0]]) if text.size else -1
+    if first == _AT:
+        return FASTQ
+    if first == _GT:
+        return FASTA
+    raise KmcB200Error(ERR_INVALID, "input is neither FASTQ ('@') nor FASTA ('>')")
+
+
+def _pinned(nbytes):
+    import torch
+    t = torch.empty(nbytes, dtype=torch.uint8, pin_memory=True)
+    return t, t.numpy()
+
+
+class _RawChunks:
+    """One file as raw chunks of at most chunk_bytes in pinned host memory, for the GPU parser.  A reader thread fills two pinned buffers
+    in turn with the next chunk_bytes / 2 bytes of the file, so reading the next piece overlaps the work on the current chunk.  Iterating
+    gives (chunk, is_final); the caller reports how much of each non-final chunk it parsed with .consumed(n), and the rest (an unfinished
+    record) is copied in front of the next piece, so every chunk starts on a record.  close() (or leaving the `with`) ends the thread."""
+
+    def __init__(self, path, chunk_bytes):
+        self.size = os.path.getsize(path)
+        self.piece = max(1, chunk_bytes // 2)
+        self.head = chunk_bytes - self.piece                           # room for the carried rest of the previous chunk
+        self.bufs = [_pinned(chunk_bytes) for _ in range(2)]
+        self.free, self.full = queue.Queue(), queue.Queue()
+        for i in range(2):
+            self.free.put(i)
+        self.wait_s = 0.0                                               # time the consumer waited for the reader
+        self._consumed = None
+        self._f = open(path, "rb")
+        self._thread = threading.Thread(target=self._read, name="kmc_b200-reader", daemon=True)
+        self._thread.start()
+
+    def _read(self):
+        try:
+            off = 0
+            while off < self.size:
+                i = self.free.get()
+                if i is None:
+                    return
+                want = min(self.piece, self.size - off)
+                n = self._f.readinto(memoryview(self.bufs[i][1])[self.head:self.head + want])
+                if n != want:
+                    raise KmcB200Error(ERR_INVALID, "short read: the file changed while it was read")
+                off += n
+                self.full.put((i, n, off >= self.size))
+        except BaseException as e:  # noqa: BLE001 - handed to the consumer
+            self.full.put(e)
+
+    def consumed(self, n):
+        self._consumed = int(n)
+
+    def __iter__(self):
+        carry = None                                                    # (buffer, start, end) of the unparsed rest
+        while self.size:
+            t = time.perf_counter()
+            item = self.full.get()
+            self.wait_s += time.perf_counter() - t
+            if isinstance(item, BaseException):
+                raise item
+            i, n, final = item
+            buf = self.bufs[i][1]
+            start = self.head
+            if carry is not None:
+                j, s, e = carry
+                if e - s > self.head:
+                    raise KmcB200Error(ERR_INVALID, "a record is longer than the chunk (%d bytes)" % (self.head + self.piece))
+                start = self.head - (e - s)
+                buf[start:self.head] = self.bufs[j][1][s:e]
+                self.free.put(j)
+            self._consumed = None
+            yield buf[start:self.head + n], final
+            if final:
+                self.free.put(i)
+                return
+            if self._consumed is None:
+                raise KmcB200Error(ERR_INVALID, "consumed() was not reported for a non-final chunk")
+            carry = (i, start + self._consumed, self.head + n)
+
+    def close(self):
+        if self._thread.is_alive():
+            self.free.put(None)
+            self.free.put(None)
+            self._thread.join()
+        self._f.close()
+
+    def __enter__(self):
+        return self
+
+    def __exit__(self, *exc):
+        self.close()
+
+
+class _Parsers:
+    """One FastxParser per format met, created on first use."""
+
+    def __init__(self, device, max_chunk_bytes):
+        self.device, self.max_chunk_bytes, self.by_format = device, max_chunk_bytes, {}
+
+    def __call__(self, chunk):
+        fmt = fastx_format(chunk)
+        if fmt not in self.by_format:
+            self.by_format[fmt] = FastxParser(fmt, self.device, self.max_chunk_bytes)
+        return self.by_format[fmt]
+
+    def close(self):
+        for p in self.by_format.values():
+            p.close()
+        self.by_format = {}
+
+
+def signature_sample_counts(paths, k, signature_len, batch_bytes=1 << 26, device=0, parse="host"):
     """Stage 0's statistics (CKMC::buildSignatureMapping, kmc_core/kmc.h:974-1075): k-mers per signature, counted on the GPU, over the
-    raw bytes of the files in input order up to the end of the first record at or beyond max(2^28, total bytes / 100)."""
-    import os
+    raw bytes of the files in input order up to the end of the first record at or beyond max(2^28, total bytes / 100).
+    parse="gpu": the files are parsed on the GPU in chunks of batch_bytes - 1, the sample's end found by the parser's limit."""
     budget = max(STATS_SAMPLE_BYTES, sum(os.path.getsize(p) for p in paths) // 100)
     st = SignatureStats(k, signature_len, device, max_batch_bytes=batch_bytes)
+    if parse == "gpu":
+        parsers = _Parsers(device, batch_bytes - 1)
+        try:
+            for path in paths:
+                if budget <= 0:
+                    break
+                size, pos = os.path.getsize(path), 0
+                with _RawChunks(path, batch_bytes - 1) as chunks:
+                    parser = None
+                    for chunk, final in chunks:
+                        parser = parser or parsers(chunk)
+                        limit = budget - pos if size > budget else None
+                        used = st.add_fastx(parser, chunk, final, limit)
+                        chunks.consumed(used)
+                        pos += used
+                        if size > budget and pos >= budget:
+                            break
+                budget -= pos
+        finally:
+            parsers.close()
+        counts = st.read()
+        st.close()
+        return counts
     for path in paths:
         if budget <= 0:
             break
@@ -123,18 +270,22 @@ def signature_sample_counts(paths, k, signature_len, batch_bytes=1 << 26, device
 
 
 def count_reads(paths, out_prefix, k, signature_len, signature_map, lut_prefix_len, cutoff_min=2, cutoff_max=1_000_000_000, counter_max=255,
-                both_strands=True, batch_bytes=1 << 26, device=0, n_bins=None):
+                both_strands=True, batch_bytes=1 << 26, device=0, n_bins=None, parse="host"):
     """KMC's stages on one GPU in RAM mode: every batch of every file is split on the GPU and the bin fragments stay in host memory;
     then bin by bin, stage 2 and the database writer.  Returns the writer's totals and the split's counts.
     With a signature_map: the bins are written in bin-id order, bin b's signatures (the map's preimage of b) go into .kmc_pre, and n_bins
     defaults to the largest map value + 1.
     With signature_map=None: stage 0 first (signature_sample_counts, then kmc_b200.signature_map with n_bins, default 512), the split
     counts the (k+x)-mers of every bin, and the bins are written in the reference's stage-2 order (kmc_b200.stage2_bin_order); the map in
-    .kmc_pre holds every signature's file position, 0 for the signatures that are not allowed."""
+    .kmc_pre holds every signature's file position, 0 for the signatures that are not allowed.
+    parse="host" reads every file whole and parses it in numpy; parse="gpu" reads chunks of batch_bytes - 1 bytes on a reader thread and
+    parses them on the GPU (kmc_b200.FastxParser, see the module docstring); the files and counts are the same either way."""
+    if parse not in ("host", "gpu"):
+        raise KmcB200Error(ERR_INVALID, "parse must be 'host' or 'gpu', not %r" % (parse,))
     t0 = time.perf_counter()
     if signature_map is None:
         n_bins = DEFAULT_N_BINS if n_bins is None else int(n_bins)
-        mapper = _signature_map(signature_sample_counts(paths, k, signature_len, batch_bytes, device), signature_len, n_bins)
+        mapper = _signature_map(signature_sample_counts(paths, k, signature_len, batch_bytes, device, parse), signature_len, n_bins)
         sig_map = np.maximum(mapper, 0).astype(np.uint32)              # no k-mer has a signature that is not allowed
     else:
         mapper = None
@@ -147,17 +298,43 @@ def count_reads(paths, out_prefix, k, signature_len, signature_map, lut_prefix_l
         sp.count_kxmers(both_strands)
     parts = [[] for _ in range(n_bins)]
     n_super = n_kmers = n_bases = 0
-    for path in paths:
-        with open(path, "rb") as f:
-            seq = sequences_to_batch(f.read())
-        for batch in batches(seq, batch_bytes):
-            out, packs, frags = sp.split_raw(batch)
-            n_bases += batch.size
-            for b, fr in enumerate(frags):
-                if fr.bytes:
-                    parts[b].append((out[fr.byte_off:fr.byte_off + fr.bytes].copy(), packs[fr.pack0:fr.pack0 + fr.n_packs].copy(), int(fr.n_rec)))
-                    n_super += int(fr.n_super_kmers)
-                    n_kmers += int(fr.n_rec)
+    read_s = 0.0
+
+    def keep(out, packs, frags):
+        nonlocal n_super, n_kmers
+        for b, fr in enumerate(frags):
+            if fr.bytes:
+                parts[b].append((out[fr.byte_off:fr.byte_off + fr.bytes].copy(), packs[fr.pack0:fr.pack0 + fr.n_packs].copy(), int(fr.n_rec)))
+                n_super += int(fr.n_super_kmers)
+                n_kmers += int(fr.n_rec)
+
+    parsers = _Parsers(device, batch_bytes - 1) if parse == "gpu" else None
+    try:
+        for path in paths:
+            if parsers is not None:
+                with _RawChunks(path, batch_bytes - 1) as chunks:
+                    parser = None
+                    for chunk, final in chunks:
+                        parser = parser or parsers(chunk)
+                        out, packs, frags, used, nseq = sp.split_fastx(parser, chunk, final)
+                        chunks.consumed(used)
+                        n_bases += nseq
+                        keep(out, packs, frags)
+                read_s += chunks.wait_s
+                continue
+            t = time.perf_counter()
+            with open(path, "rb") as f:
+                data = f.read()
+            read_s += time.perf_counter() - t
+            seq = sequences_to_batch(data)
+            del data
+            for batch in batches(seq, batch_bytes):
+                out, packs, frags = sp.split_raw(batch)
+                n_bases += batch.size
+                keep(out, packs, frags)
+    finally:
+        if parsers is not None:
+            parsers.close()
     if mapper is None:
         file_order = np.arange(n_bins)
         order = np.argsort(sig_map, kind="stable")
@@ -192,7 +369,7 @@ def count_reads(paths, out_prefix, k, signature_len, signature_map, lut_prefix_l
     ctx.close()
     t2 = time.perf_counter()
     return {"n_unique": totals[0], "n_cutoff_min": totals[1], "n_cutoff_max": totals[2], "n_total": totals[3], "n_super_kmers": n_super,
-            "n_kmers": n_kmers, "n_bases": n_bases, "stats_s": t_stats, "split_s": t1 - t0 - t_stats, "stage2_s": t2 - t1}
+            "n_kmers": n_kmers, "n_bases": n_bases, "stats_s": t_stats, "split_s": t1 - t0 - t_stats, "stage2_s": t2 - t1, "read_s": read_s}
 
 
 def main(argv=None):
@@ -210,6 +387,7 @@ def main(argv=None):
     ap.add_argument("-b", action="store_true", help="count k-mers as they are, not canonical ones")
     ap.add_argument("--batch-bytes", type=int, default=1 << 26)
     ap.add_argument("--device", type=int, default=0)
+    ap.add_argument("--gpu-parse", action="store_true", help="parse FASTQ / FASTA on the GPU in chunks of batch-bytes - 1 (default: numpy, whole files)")
     a = ap.parse_args(argv)
     if len(a.inputs) < 2:
         ap.error("give at least one input and the output prefix")
@@ -223,7 +401,7 @@ def main(argv=None):
     if lp is None:
         lp = next(p for p in (7, 3, 11, 15, 4, 5, 6, 2, 8, 9, 10, 12, 13, 14, 1) if p < a.k and (a.k - p) % 4 == 0)
     res = count_reads(a.inputs[:-1], a.inputs[-1], a.k, m, sig_map, lp, a.ci, a.cx, a.cs, not a.b, a.batch_bytes, a.device,
-                      a.n_bins if sig_map is None else None)
+                      a.n_bins if sig_map is None else None, parse="gpu" if a.gpu_parse else "host")
     print(json.dumps(res))
     return 0
 

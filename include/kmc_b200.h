@@ -21,9 +21,12 @@
  * Environment knobs read by kmcb200_create (development / tests; the defaults are the measured best):
  *   KMCB200_SORT=lsd               plain 8-bit LSD passes instead of the hybrid MSD sort
  *   KMCB200_LEAF=sort              sort the leaves on chip + count_emit instead of counting them in hash tables
- *   KMCB200_LEAF_SLOT_BITS=8|9|10  slots of a warp's leaf table (default 10)
- *   KMCB200_LEAF_KERNEL=warp       round 1's leaf kernel (ordered groups, leaf_warp.cuh) instead of leaf_hash_kernel; KMCB200_LEAF_WIDE=warp: for records of > 1 word only
- *   KMCB200_LEAF_FILL_PCT=n        leaf_hash_kernel plans a table round for this load (default 62); KMCB200_LEAF_RATIO0=n: first guess of distinct k-mers per record x 256 (default 90)
+ *   KMCB200_LEAF_SLOT_BITS=8|9|10  slots of a warp's leaf table (default 10; not leaf_hash_cta_kernel's: KMCB200_LEAF_CTA)
+ *   KMCB200_LEAF_KERNEL=cta|hash|warp  one-word records always by one table per CTA (leaf_hash_cta_kernel) / one table per warp (leaf_hash_kernel) /
+ *                                  round 1's leaf kernel (ordered groups, leaf_warp.cuh); default: the CTA kernel in bins whose mean leaf is > 1280
+ *                                  records, leaf_hash_kernel below; KMCB200_LEAF_WIDE=warp: round 1's kernel for records of > 1 word
+ *   KMCB200_LEAF_CTA=W:B           leaf_hash_cta_kernel: W warps per CTA share one table of 2^B slots; 4:12 (default), 8:12, 8:13 or 4:10
+ *   KMCB200_LEAF_FILL_PCT=n        the hash kernels plan a table round for this load (default 62); KMCB200_LEAF_RATIO0=n: first guess of distinct k-mers per record x 256 (default 90)
  *   KMCB200_LEAF_ROUND_PCT=n       leaf_warp_kernel: records per table round in percent of the slots (default 100)
  *   KMCB200_L2_BITS=1..10          bits of the second partition level (default: from the bin size: 8 for one-word records; wider records up to 10)
  *   KMCB200_LEAF_TARGET=n, KMCB200_LEAF_MAX_B2=8..10   mean leaf size / most bits the default rule aims at for one-word records (1024, 8)

@@ -11,6 +11,7 @@
 #include "msd_sort.cuh"
 #include "leaf_warp.cuh"
 #include "leaf_hash.cuh"
+#include "leaf_hash_cta.cuh"
 #include "leaf_hash_wide.cuh"
 #include "split.cuh"
 #include "fastx.cuh"
@@ -140,6 +141,10 @@ struct kmcb200_ctx {
 	int occ_leaf_hash = 1;
 	bool leaf_hash_wide = true;                             // KMCB200_LEAF_WIDE = hash | warp: records of more than one word by leaf_hash_wide_kernel / leaf_warp_kernel
 	bool leaf_hash = true;                                  // KMCB200_LEAF_KERNEL = hash | warp: one-word records are counted by leaf_hash_kernel (round 2) / leaf_warp_kernel
+	int leaf_cta = 2;                                       // one-word records by leaf_hash_cta_kernel (one table per CTA): 2 = in bins of mean leaves > kLeafCtaMinMean,
+	                                                        // 1 = always (KMCB200_LEAF_KERNEL=cta), 0 = never (KMCB200_LEAF_KERNEL = hash | warp)
+	int leaf_cta_warps = 4, leaf_cta_slot_bits = 12;        // KMCB200_LEAF_CTA = W:B, its warps per CTA and table slots (2^B)
+	int occ_leaf_cta = 1;
 	uint32_t leaf_max_b2 = 8;                               // KMCB200_LEAF_MAX_B2 (8: on the H100 the 512 / 1024-digit level 2 costs more than it saves, DESIGN 3.1)
 	uint32_t leaf_target = 1024;                            // KMCB200_LEAF_TARGET: mean leaf size the second partition level of a large bin aims at (leaf_hash_kernel)
 	uint32_t leaf_fill_pct = 62;                            // KMCB200_LEAF_FILL_PCT: leaf_hash_kernel plans a table round for this load
@@ -722,8 +727,43 @@ __global__ void finish_result_kernel(uint64_t* result, uint64_t n_rec, const uin
 	}
 }
 
+// leaf_hash_cta_kernel: one instance per setting of KMCB200_LEAF_CTA (warps per CTA : log2 of the table's slots)
+template <int NWARPS, int SLOT_BITS>
+int launch_leaf_cta(kmcb200_ctx* ctx, const LeafArgs& la, bool simple, cudaStream_t st)
+{
+	const size_t smem = sizeof(LcSmem<NWARPS, SLOT_BITS>);
+	const uint32_t grid = std::min<uint32_t>(la.n_leaves, (uint32_t)(ctx->sm_count * ctx->occ_leaf_cta));
+	if (simple) leaf_hash_cta_kernel<NWARPS, SLOT_BITS, true><<<grid, 32 * NWARPS, smem, st>>>(la);
+	else leaf_hash_cta_kernel<NWARPS, SLOT_BITS, false><<<grid, 32 * NWARPS, smem, st>>>(la);
+	return 0;
+}
+
+template <int NWARPS, int SLOT_BITS>
+int setup_leaf_cta(kmcb200_ctx* ctx)
+{
+	const int smem = (int)sizeof(LcSmem<NWARPS, SLOT_BITS>);
+	int occ_t = 1, occ_f = 1;
+	CU((cudaFuncSetAttribute(leaf_hash_cta_kernel<NWARPS, SLOT_BITS, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem)));
+	CU((cudaFuncSetAttribute(leaf_hash_cta_kernel<NWARPS, SLOT_BITS, true>, cudaFuncAttributePreferredSharedMemoryCarveout, 100)));
+	CU((cudaFuncSetAttribute(leaf_hash_cta_kernel<NWARPS, SLOT_BITS, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem)));
+	CU((cudaFuncSetAttribute(leaf_hash_cta_kernel<NWARPS, SLOT_BITS, false>, cudaFuncAttributePreferredSharedMemoryCarveout, 100)));
+	CU((cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ_t, leaf_hash_cta_kernel<NWARPS, SLOT_BITS, true>, 32 * NWARPS, smem)));
+	CU((cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ_f, leaf_hash_cta_kernel<NWARPS, SLOT_BITS, false>, 32 * NWARPS, smem)));
+	ctx->occ_leaf_cta = std::max(1, std::min(occ_t, occ_f));
+	return 0;
+}
+
+// leaf_hash_cta_kernel takes the bins whose mean leaf (records / leaves) is larger than this.  Its gain is that a leaf of up to ~8 K records
+// of a 30x bin is one table round where a warp's table needs 2 .. 4 (leaves spread over 0 .. 2x their mean; a warp's round holds ~1800
+// records); for leaves that already fit one warp round, the warp kernel's independent warps are faster (DESIGN 3.2: 0.58 against
+// 0.77 ms for a 2^26-k-mer bin, mean leaf 1024, on an H100).
+constexpr uint64_t kLeafCtaMinMean = 1280;
+
+#define DISPATCH_CTA(ctx, fn, ...) ((ctx)->leaf_cta_warps == 8 ? ((ctx)->leaf_cta_slot_bits == 13 ? fn<8, 13>(__VA_ARGS__) : fn<8, 12>(__VA_ARGS__)) \
+                                                             : ((ctx)->leaf_cta_slot_bits == 10 ? fn<4, 10>(__VA_ARGS__) : fn<4, 12>(__VA_ARGS__)))
+
 template <int WORDS, int SLOT_BITS>
-int launch_leaves(kmcb200_ctx* ctx, const LeafArgs& la, cudaStream_t st)
+int launch_leaves(kmcb200_ctx* ctx, const LeafArgs& la, uint64_t n_rec, cudaStream_t st)
 {
 	if (ctx->leaf_hash && (WORDS == 1 || ctx->leaf_hash_wide)) {
 		const size_t hsmem = sizeof(LhSmem<SLOT_BITS>) * kLwWarps;
@@ -732,7 +772,8 @@ int launch_leaves(kmcb200_ctx* ctx, const LeafArgs& la, cudaStream_t st)
 		const uint32_t max_count = WORDS == 1 ? kLwHeavy : kLwMaxLeaf;
 		const bool simple = la.cutoff_min >= 2u && la.cutoff_max >= la.cutoff_min && (la.cutoff_max + 1u == 0u || la.cutoff_max + 1u > max_count + 1u);
 		if constexpr (WORDS == 1) {
-			if (simple) leaf_hash_kernel<SLOT_BITS, true><<<hgrid, 32 * kLwWarps, hsmem, st>>>(la);
+			if (ctx->leaf_cta == 1 || (ctx->leaf_cta == 2 && n_rec > kLeafCtaMinMean * la.n_leaves)) DISPATCH_CTA(ctx, launch_leaf_cta, ctx, la, simple, st);
+			else if (simple) leaf_hash_kernel<SLOT_BITS, true><<<hgrid, 32 * kLwWarps, hsmem, st>>>(la);
 			else leaf_hash_kernel<SLOT_BITS, false><<<hgrid, 32 * kLwWarps, hsmem, st>>>(la);
 		} else {
 			if (simple) leaf_hash_wide_kernel<WORDS, SLOT_BITS, true><<<hgrid, 32 * kLwWarps, hsmem, st>>>(la);
@@ -779,6 +820,8 @@ int setup_leaves(kmcb200_ctx* ctx)
 			CU((cudaFuncSetAttribute(leaf_hash_kernel<SLOT_BITS, false>, cudaFuncAttributePreferredSharedMemoryCarveout, 100)));
 			CU((cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ_t, leaf_hash_kernel<SLOT_BITS, true>, 32 * kLwWarps, hsmem)));
 			CU((cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ_f, leaf_hash_kernel<SLOT_BITS, false>, 32 * kLwWarps, hsmem)));
+			if (ctx->leaf_cta)
+				if (int rc = DISPATCH_CTA(ctx, setup_leaf_cta, ctx)) return rc;
 		} else {
 			CU((cudaFuncSetAttribute(leaf_hash_wide_kernel<WORDS, SLOT_BITS, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, hsmem)));
 			CU((cudaFuncSetAttribute(leaf_hash_wide_kernel<WORDS, SLOT_BITS, true>, cudaFuncAttributePreferredSharedMemoryCarveout, 100)));
@@ -833,7 +876,7 @@ int run_sort_count_leaves(kmcb200_ctx* ctx, Slot& s, uint64_t n_rec, uint32_t np
 	la.counter_max = ctx->prm.counter_max; la.counter_bytes = ctx->counter_bytes; la.suffix_bytes = ctx->suffix_bytes;
 	la.heavy_list = s.zero->heavy_list; la.heavy_count = &s.zero->heavy_count[0]; la.heavy_ticket = &s.zero->heavy_count[1]; la.heavy_cap = kHeavyListCap;
 	la.tmp = s.leaf_tmp; la.leaf_emit = s.leaf_emit; la.group_sum = s.zero->leaf_group_sum; la.lut = d_lut; la.result = d_result; la.ticket = &s.zero->msd_counters[3]; la.flags = flags;
-	if (int rc = DISPATCH_SLOTS(ctx, launch_leaves, WORDS, ctx, la, st)) return rc;
+	if (int rc = DISPATCH_SLOTS(ctx, launch_leaves, WORDS, ctx, la, n_rec, st)) return rc;
 	if (WORDS == 1) {          // the large leaves the main launch only noted (none in a typical bin: the launch returns at once)
 		if (int rc = DISPATCH_SLOTS(ctx, launch_heavy_leaves, WORDS, ctx, la, st)) return rc;
 	}
@@ -1215,7 +1258,11 @@ int kmcb200_create(const kmcb200_params* prm, kmcb200_ctx** out_ctx)
 	if (const char* e = getenv("KMCB200_MAX_CHUNK_BYTES")) { const long long v = atoll(e); if (v >= (1 << 17) && v < (1ll << 31)) ctx->max_chunk_bytes = (uint64_t)v; }
 	if (const char* e = getenv("KMCB200_L2_BITS")) { const int v = atoi(e); if (v >= 1 && v <= 10) ctx->force_b2 = (uint32_t)v; }
 	if (const char* e = getenv("KMCB200_LEAF_ROUND_PCT")) { const int v = atoi(e); if (v >= 50 && v <= 1000) ctx->leaf_round_pct = (uint32_t)v; }
-	if (const char* e = getenv("KMCB200_LEAF_KERNEL")) ctx->leaf_hash = std::string(e) != "warp";
+	if (const char* e = getenv("KMCB200_LEAF_KERNEL")) { const std::string v(e); ctx->leaf_hash = v != "warp"; ctx->leaf_cta = v == "cta" ? 1 : v == "warp" || v == "hash" ? 0 : 2; }
+	if (const char* e = getenv("KMCB200_LEAF_CTA")) {
+		const std::string v(e);
+		if (v == "4:10" || v == "4:12" || v == "8:12" || v == "8:13") { ctx->leaf_cta_warps = v[0] - '0'; ctx->leaf_cta_slot_bits = atoi(v.c_str() + 2); }
+	}
 	if (const char* e = getenv("KMCB200_LEAF_WIDE")) ctx->leaf_hash_wide = std::string(e) != "warp";
 	if (const char* e = getenv("KMCB200_LEAF_MAX_B2")) { const int v = atoi(e); if (v >= 8 && v <= 10) ctx->leaf_max_b2 = (uint32_t)v; }
 	if (const char* e = getenv("KMCB200_LEAF_TARGET")) { const int v = atoi(e); if (v >= 128 && v <= 8192) ctx->leaf_target = (uint32_t)v; }

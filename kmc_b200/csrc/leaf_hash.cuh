@@ -193,19 +193,28 @@ __device__ __forceinline__ void lh_drain(const LhRound& t, uint32_t& head, uint3
 	}
 }
 
-// the insertion of one round: 4 k-mers per lane and step, first probes of all four before any result is looked at; returns false when the
-// table fills up (more distinct k-mers than planned).  MULTI: one of several rounds of a leaf - only the k-mers whose next bits are r
-template <int SLOT_BITS, bool SIMPLE, bool MULTI>
-__device__ __forceinline__ bool lh_insert(const LhRound& T, const unsigned long long* __restrict__ g, uint32_t m, uint32_t kb, uint32_t emask, uint32_t r,
-	uint32_t limit, uint32_t lane, uint32_t lt, uint32_t& r_claim, uint32_t& r_max)
+// when a round's table is full: asked after every step that may have claimed slots (a full table must end the round there, or probes
+// would circulate in the queue for ever).  The warp kernel owns its table: its lanes' claims of the round are the whole count.
+struct LhWarpCtl {
+	static constexpr uint32_t kStride = 128;             // records between two steps of a warp
+	uint32_t limit;
+	__device__ __forceinline__ bool full(uint32_t& r_claim) const { return __reduce_add_sync(0xffffffffu, r_claim) > limit; }
+};
+
+// the insertion of one round: 4 k-mers per lane and step (records first + 128 * i .. + 127, stepping by Ctl::kStride), first probes of all
+// four before any result is looked at; returns false when the table fills up (more distinct k-mers than planned).  MULTI: one of several
+// rounds of a leaf - only the k-mers whose next bits are r
+template <int SLOT_BITS, bool SIMPLE, bool MULTI, class Ctl>
+__device__ __forceinline__ bool lh_insert(const LhRound& T, const Ctl& ctl, const unsigned long long* __restrict__ g, uint32_t first, uint32_t m, uint32_t kb,
+	uint32_t emask, uint32_t r, uint32_t lane, uint32_t lt, uint32_t& r_claim, uint32_t& r_max)
 {
 	constexpr uint32_t FULL = 0xffffffffu;
 	uint32_t head = 0, tail = 0;
 	bool ok = true;
 	uint64_t nx[4];
 #pragma unroll
-	for (int u = 0; u < 4; ++u) { const uint32_t j = u * 32 + lane; nx[u] = j < m ? __ldg(g + j) : 0ull; }
-	for (uint32_t j0 = 0; j0 < m; j0 += 128) {
+	for (int u = 0; u < 4; ++u) { const uint32_t j = first + u * 32 + lane; nx[u] = j < m ? __ldg(g + j) : 0ull; }
+	for (uint32_t j0 = first; j0 < m; j0 += Ctl::kStride) {
 		uint64_t rem[4];
 		uint32_t slot[4];
 		unsigned long long ent[4], old[4];
@@ -221,7 +230,7 @@ __device__ __forceinline__ bool lh_insert(const LhRound& T, const unsigned long 
 			old[u] = lh_probe(act[u], T.s_main + slot[u] * 8u, T.s_dummy, ent[u]);
 		}
 #pragma unroll
-		for (int u = 0; u < 4; ++u) { const uint32_t j = j0 + 128 + u * 32 + lane; nx[u] = j < m ? __ldg(g + j) : 0ull; }
+		for (int u = 0; u < 4; ++u) { const uint32_t j = j0 + Ctl::kStride + u * 32 + lane; nx[u] = j < m ? __ldg(g + j) : 0ull; }
 #pragma unroll
 		for (int u = 0; u < 4; ++u) {
 			const bool miss = lh_settle<SIMPLE>(T, act[u], old[u], ent[u], slot[u], r_claim, r_max);
@@ -229,11 +238,10 @@ __device__ __forceinline__ bool lh_insert(const LhRound& T, const unsigned long 
 			if (miss) T.queue[(tail + __popc(bal & lt)) & (kLhQueue - 1)] = (1ull << kLhKeyBits) | rem[u];
 			tail += __popc(bal);
 		}
-		// (a table that fills up must end the round HERE: probes into a full table would circulate in the queue for ever)
-		if (__reduce_add_sync(FULL, r_claim) > limit) ok = false;          // more distinct k-mers than planned: the round is split
+		if (ctl.full(r_claim)) ok = false;          // more distinct k-mers than planned: the round is split
 		while (ok && tail - head >= 64u) {
 			lh_drain<SLOT_BITS, SIMPLE>(T, head, tail, lane, lt, r_claim, r_max);
-			if (__reduce_add_sync(FULL, r_claim) > limit) ok = false;
+			if (ctl.full(r_claim)) ok = false;
 		}
 		if (!ok) break;
 	}
@@ -252,7 +260,7 @@ __device__ __forceinline__ bool lh_insert(const LhRound& T, const unsigned long 
 			const unsigned long long old = lh_probe(pend, T.s_main + slot * 8u, T.s_dummy, ent);
 			pend = lh_settle<SIMPLE>(T, pend, old, ent, slot, r_claim, r_max);
 			slot = (slot + 1u) & ((1u << SLOT_BITS) - 1u);
-			if (__reduce_add_sync(FULL, r_claim) > limit) { ok = false; break; }          // (a full table would keep the loop going for ever)
+			if (ctl.full(r_claim)) { ok = false; break; }          // (a full table would keep the loop going for ever)
 			if (!__any_sync(FULL, pend)) break;
 		}
 	}
@@ -337,8 +345,9 @@ __global__ void __launch_bounds__(32 * kLwWarps, KMCB200_LH_MINBLOCKS) leaf_hash
 				const LhRound T{smem_u32(S.main), smem_u32(S.queue), smem_u32(S.surv), smem_u32(S.over), smem_u32(&S.dummy[lane]), S.queue, cb, cmask, rem_mask, 1ull << cb,
 					cut.cmin, cut.cmax1, cut.never, cut.cmax1 != 0u && cut.cmax1 <= kLwHeavy + 1u};
 				uint32_t r_claim = 0, r_max = 0;
-				const bool ok = e == 0 ? lh_insert<SLOT_BITS, SIMPLE, false>(T, g, m, kb, emask, r, LIMIT, lane, lt, r_claim, r_max)
-				                       : lh_insert<SLOT_BITS, SIMPLE, true>(T, g, m, kb, emask, r, LIMIT, lane, lt, r_claim, r_max);
+				const LhWarpCtl ctl{LIMIT};
+				const bool ok = e == 0 ? lh_insert<SLOT_BITS, SIMPLE, false>(T, ctl, g, 0u, m, kb, emask, r, lane, lt, r_claim, r_max)
+				                       : lh_insert<SLOT_BITS, SIMPLE, true>(T, ctl, g, 0u, m, kb, emask, r, lane, lt, r_claim, r_max);
 				if (!prefetched) {        // the next leaf: towards L2 while this one is counted
 					prefetched = true;
 					const uint32_t nl = __shfl_sync(FULL, next_t, 0);

@@ -319,6 +319,58 @@ int kmcb200_split_fastx(kmcb200_splitter* sp, kmcb200_fastx* p, const uint8_t* r
 int kmcb200_sigstats_add_fastx(kmcb200_sigstats* h, kmcb200_fastx* p, const uint8_t* raw, uint64_t bytes, int is_final, uint64_t limit,
 	uint64_t* consumed);
 
+/* ---- small k: reads -> direct counts -> KMC1 database (KMC's small-k mode, kmc_core/kmc.h:677-960) -------------------------------
+ * For k <= 13 the reference builds no bins: it counts every k-mer in a direct array of 4^k uint64 counters (CSplitter::ProcessReadsSmallK,
+ * splitter.cpp:681-805) and writes a KMC1-format database from it (CSmallKCompleter::CompleteKMCFormat, kb_completer.h:148-308).
+ *   counting  the batch format is kmcb200_split's; every k-mer of ACGT only adds 1 to counts[v], v = its 2k-bit code (first symbol most
+ *             significant), or min(code, reverse complement) with both strands.  Counts add up over calls until reset.
+ *   finish    n_unique (non-zero counters), n_cutoff_min (count < cutoff_min), n_cutoff_max (count > cutoff_max), n_total (sum of the
+ *             counts), and the LUT prefix length lp of 1..15 with (k - lp) % 4 == 0 of least n_unique * ((k - lp) / 4 + calc_counter_size)
+ *             + 8 * 4^lp (kmc.h:906-936).  Records are (k - lp) / 4 suffix bytes (most significant first) and min(count, counter_max) in
+ *             counter_size bytes (least significant first), counter_size = calc_counter_size_ull (defs.h:161), 0 when counter_max == 1.
+ *   emit      the records of the kept k-mers in k-mer order, and lut[4^lp]: lut[p] = kept k-mers whose prefix is below p (no sentinel).
+ *   write_db  finish + emit + the two files: .kmc_suf "KMCS" records "KMCS"; .kmc_pre "KMCP" lut, the KMC1 footer (version word 0, no
+ *             signature map) and "KMCP".
+ * Work: 1 launch per add, 4 per finish (one synchronisation), 1 per emit.  Workspace: the batch (max_batch_bytes, host path), the 4^k
+ * counters (512 MiB at k = 13), one word per 4096 counters, and the records and LUT of an emit. */
+typedef struct kmcb200_smallk kmcb200_smallk;
+typedef struct {
+	uint32_t kmer_len;                    /* 1..13 */
+	uint32_t both_strands;                /* 1: canonical k-mers, 0: as they are (-b) */
+	int32_t device;                       /* CUDA ordinal */
+	uint32_t reserved;                    /* 0 */
+	uint64_t max_batch_bytes;             /* largest batch one call accepts (1..KMCB200_SPLIT_MAX_BATCH) */
+} kmcb200_smallk_params;
+/* KMCB200_ERR_INVALID for a bad parameter, KMCB200_ERR_NO_DEVICE without an sm_90 device (no CPU fallback).  The counters start at 0. */
+int kmcb200_smallk_create(const kmcb200_smallk_params* params, kmcb200_smallk** out);
+void kmcb200_smallk_destroy(kmcb200_smallk* h);
+/* message of the last failure on this handle (or of the last failed create when h == NULL) */
+const char* kmcb200_smallk_last_error(const kmcb200_smallk* h);
+/* Number of kernels this handle has launched so far. */
+uint64_t kmcb200_smallk_kernel_launches(const kmcb200_smallk* h);
+/* Host batch: copied in, counted; returns when the batch buffer may be reused.  A batch over max_batch_bytes: KMCB200_ERR_INVALID. */
+int kmcb200_smallk_add(kmcb200_smallk* h, const uint8_t* seq, uint64_t bytes);
+/* Device twin: d_seq in HBM, queued on `stream` (a cudaStream_t; NULL = the legacy default stream) after the handle's earlier work. */
+int kmcb200_dev_smallk_add(kmcb200_smallk* h, const uint8_t* d_seq, uint64_t bytes, void* stream);
+/* kmcb200_smallk_add of a raw FASTQ / FASTA chunk parsed on the GPU straight into the handle's batch buffer (see kmcb200_fastx_parse for
+ * is_final and *consumed; *seq_bytes, which may be NULL, receives the batch's length).  bytes + 1 > max_batch_bytes:
+ * KMCB200_ERR_INVALID.  Errors are reported on the counter handle. */
+int kmcb200_smallk_add_fastx(kmcb200_smallk* h, kmcb200_fastx* p, const uint8_t* raw, uint64_t bytes, int is_final, uint64_t* consumed,
+	uint64_t* seq_bytes);
+/* counts[4^k] (host) after every call queued so far, device twin included. */
+int kmcb200_smallk_read(kmcb200_smallk* h, uint64_t* counts);
+int kmcb200_smallk_reset(kmcb200_smallk* h);
+/* The totals and the layout of the database of the current counts: *lut_prefix_len, *counter_size, *suffix_bytes (the bytes of all the
+ * records), stats[4] = n_unique, n_cutoff_min, n_cutoff_max, n_total.  A k-mer is kept when cutoff_min <= count <= cutoff_max. */
+int kmcb200_smallk_finish(kmcb200_smallk* h, uint32_t cutoff_min, uint64_t cutoff_max, uint64_t counter_max, uint32_t* lut_prefix_len,
+	uint32_t* counter_size, uint64_t* suffix_bytes, uint64_t* stats);
+/* After finish (and no add or reset since): suffix[0, suffix_bytes) the records, lut[4^lut_prefix_len] the LUT.  capacity < suffix_bytes:
+ * KMCB200_ERR_CAPACITY and nothing is written; no finish: KMCB200_ERR_INVALID. */
+int kmcb200_smallk_emit(kmcb200_smallk* h, uint8_t* suffix, uint64_t capacity, uint64_t* lut);
+/* finish + emit + path_prefix.kmc_pre / path_prefix.kmc_suf; totals[4] as finish's stats. */
+int kmcb200_smallk_write_db(kmcb200_smallk* h, const char* path_prefix, uint32_t cutoff_min, uint64_t cutoff_max, uint64_t counter_max,
+	uint64_t* totals);
+
 /* ---- seam #1: sort host records ------------------------------------------------------------------
  * Contract of SortFunction (raduls.h:19-20, kb_sorter.h:775-779): n records of rec_bytes (multiple of 8,
  * CKmer<SIZE> images) sorted ascending on bytes key_bytes-1..0; the result is left in `tmp` when key_bytes

@@ -43,6 +43,10 @@ class _SigstatsParams(C.Structure):
     _fields_ = [("kmer_len", C.c_uint32), ("signature_len", C.c_uint32), ("device", C.c_int32), ("reserved", C.c_uint32), ("max_batch_bytes", C.c_uint64)]
 
 
+class _SmallKParams(C.Structure):
+    _fields_ = [("kmer_len", C.c_uint32), ("both_strands", C.c_uint32), ("device", C.c_int32), ("reserved", C.c_uint32), ("max_batch_bytes", C.c_uint64)]
+
+
 class _FastxParams(C.Structure):
     _fields_ = [("device", C.c_int32), ("format", C.c_uint32), ("max_chunk_bytes", C.c_uint64)]
 
@@ -65,6 +69,9 @@ EXPORTS = [
     "kmcb200_sigstats_read", "kmcb200_sigstats_reset", "kmcb200_sigstats_kernel_launches", "kmcb200_signature_map", "kmcb200_stage2_bin_order",
     "kmcb200_fastx_create", "kmcb200_fastx_destroy", "kmcb200_fastx_last_error", "kmcb200_fastx_kernel_launches", "kmcb200_fastx_parse",
     "kmcb200_dev_fastx_parse", "kmcb200_split_fastx", "kmcb200_sigstats_add_fastx",
+    "kmcb200_smallk_create", "kmcb200_smallk_destroy", "kmcb200_smallk_last_error", "kmcb200_smallk_kernel_launches", "kmcb200_smallk_add",
+    "kmcb200_dev_smallk_add", "kmcb200_smallk_add_fastx", "kmcb200_smallk_read", "kmcb200_smallk_reset", "kmcb200_smallk_finish",
+    "kmcb200_smallk_emit", "kmcb200_smallk_write_db",
 ]
 
 FASTQ, FASTA = 1, 2                                                     # KMCB200_FASTQ / KMCB200_FASTA
@@ -155,6 +162,21 @@ def load_library(build_if_needed=True):
     L.kmcb200_dev_fastx_parse.argtypes = [vp, vp, u64, C.c_int, u64, vp, u64, vp, vp]
     L.kmcb200_split_fastx.argtypes = [vp, vp, vp, u64, C.c_int, vp, u64, C.POINTER(u64), vp, u64, C.POINTER(u64), vp, C.POINTER(u64), C.POINTER(u64)]
     L.kmcb200_sigstats_add_fastx.argtypes = [vp, vp, vp, u64, C.c_int, u64, C.POINTER(u64)]
+    L.kmcb200_smallk_create.argtypes = [C.POINTER(_SmallKParams), C.POINTER(vp)]
+    L.kmcb200_smallk_destroy.argtypes = [vp]
+    L.kmcb200_smallk_destroy.restype = None
+    L.kmcb200_smallk_last_error.argtypes = [vp]
+    L.kmcb200_smallk_last_error.restype = C.c_char_p
+    L.kmcb200_smallk_kernel_launches.argtypes = [vp]
+    L.kmcb200_smallk_kernel_launches.restype = u64
+    L.kmcb200_smallk_add.argtypes = [vp, vp, u64]
+    L.kmcb200_dev_smallk_add.argtypes = [vp, vp, u64, vp]
+    L.kmcb200_smallk_add_fastx.argtypes = [vp, vp, vp, u64, C.c_int, C.POINTER(u64), C.POINTER(u64)]
+    L.kmcb200_smallk_read.argtypes = [vp, vp]
+    L.kmcb200_smallk_reset.argtypes = [vp]
+    L.kmcb200_smallk_finish.argtypes = [vp, u32, u64, u64, C.POINTER(u32), C.POINTER(u32), C.POINTER(u64), vp]
+    L.kmcb200_smallk_emit.argtypes = [vp, vp, u64, vp]
+    L.kmcb200_smallk_write_db.argtypes = [vp, C.c_char_p, u32, u64, u64, vp]
     _lib = L
     return L
 
@@ -528,6 +550,93 @@ class SignatureStats:
 
     def reset(self):
         self._check(self.lib.kmcb200_sigstats_reset(self._h))
+
+
+class SmallKCounter:
+    """Small k (1..13) on one GPU (kmcb200_smallk_*), KMC's small-k mode (kmc_core/kmc.h:677-960): every k-mer of the batches counted in
+    a direct array of 4^k uint64 counters (CSplitter::ProcessReadsSmallK), then a KMC1-format database (CSmallKCompleter).  Batches as for
+    Splitter; the counts add up until reset().  There are no bins, so no signature length, map or caller-chosen LUT prefix length: finish()
+    picks the LUT prefix length as the reference does."""
+
+    def __init__(self, kmer_len, both_strands=True, device=0, max_batch_bytes=1 << 26):
+        self.lib = load_library()
+        self.kmer_len, self.both_strands, self.max_batch_bytes = kmer_len, bool(both_strands), max_batch_bytes
+        self._h = C.c_void_p(None)
+        p = _SmallKParams(kmer_len, int(bool(both_strands)), device, 0, max_batch_bytes)
+        rc = self.lib.kmcb200_smallk_create(C.byref(p), C.byref(self._h))
+        if rc != 0:
+            raise KmcB200Error(rc, (self.lib.kmcb200_smallk_last_error(None) or b"").decode())
+
+    def _check(self, rc):
+        if rc < 0:
+            raise KmcB200Error(rc, (self.lib.kmcb200_smallk_last_error(self._h) or b"").decode())
+        return rc
+
+    def close(self):
+        if self._h:
+            self.lib.kmcb200_smallk_destroy(self._h)
+            self._h = C.c_void_p(None)
+
+    def __del__(self):
+        try:
+            self.close()
+        except Exception:
+            pass
+
+    def kernel_launches(self):
+        return int(self.lib.kmcb200_smallk_kernel_launches(self._h))
+
+    def add(self, batch):
+        seq = _as_u8(batch)
+        self._check(self.lib.kmcb200_smallk_add(self._h, seq.ctypes.data, seq.size))
+
+    def dev_add(self, d_seq, nbytes, stream=None):
+        """kmcb200_dev_smallk_add: d_seq a device pointer (int or a tensor's data_ptr()), queued on `stream` (a cudaStream_t)."""
+        self._check(self.lib.kmcb200_dev_smallk_add(self._h, d_seq, nbytes, stream))
+
+    def add_fastx(self, parser, raw, is_final=True):
+        """kmcb200_smallk_add_fastx: a raw FASTQ / FASTA chunk parsed on the GPU by `parser` and counted.  Returns `consumed`, the bytes
+        parsed (the caller carries the rest into its next chunk); the length of the batch the chunk gave is left in last_seq_bytes."""
+        a = _as_u8(raw)
+        consumed, seq_bytes = C.c_uint64(0), C.c_uint64(0)
+        self._check(self.lib.kmcb200_smallk_add_fastx(self._h, parser._h, a.ctypes.data, a.size, int(bool(is_final)), C.byref(consumed),
+                                                      C.byref(seq_bytes)))
+        self.last_seq_bytes = int(seq_bytes.value)
+        return int(consumed.value)
+
+    def read(self):
+        """uint64[4^k]: the counts of every k-mer value so far."""
+        out = np.zeros(1 << (2 * self.kmer_len), dtype=np.uint64)
+        self._check(self.lib.kmcb200_smallk_read(self._h, out.ctypes.data))
+        return out
+
+    def reset(self):
+        self._check(self.lib.kmcb200_smallk_reset(self._h))
+
+    def finish(self, cutoff_min=2, cutoff_max=1_000_000_000, counter_max=255):
+        """kmcb200_smallk_finish: (lut_prefix_len, counter_size, suffix_bytes, (n_unique, n_cutoff_min, n_cutoff_max, n_total))."""
+        lp, cs, nbytes = C.c_uint32(0), C.c_uint32(0), C.c_uint64(0)
+        st = (C.c_uint64 * 4)()
+        self._check(self.lib.kmcb200_smallk_finish(self._h, cutoff_min, min(int(cutoff_max), (1 << 64) - 1), min(int(counter_max), (1 << 64) - 1),
+                                                   C.byref(lp), C.byref(cs), C.byref(nbytes), st))
+        self._layout = (int(lp.value), int(nbytes.value))
+        return int(lp.value), int(cs.value), int(nbytes.value), tuple(int(x) for x in st)
+
+    def emit(self, out=None):
+        """kmcb200_smallk_emit after finish(): (records, lut).  `out` (uint8, default: exactly suffix_bytes fresh bytes) receives the records;
+        a shorter one raises ERR_CAPACITY and is left untouched."""
+        lp, nbytes = getattr(self, "_layout", (0, 0))
+        o = np.empty(nbytes, dtype=np.uint8) if out is None else out
+        lut = np.empty(1 << (2 * lp), dtype=np.uint64)
+        self._check(self.lib.kmcb200_smallk_emit(self._h, o.ctypes.data if o.size else None, o.size, lut.ctypes.data))
+        return o[:nbytes], lut
+
+    def write_db(self, path_prefix, cutoff_min=2, cutoff_max=1_000_000_000, counter_max=255):
+        """kmcb200_smallk_write_db: path_prefix.kmc_pre / .kmc_suf in KMC1 format; returns (n_unique, n_cutoff_min, n_cutoff_max, n_total)."""
+        tot = (C.c_uint64 * 4)()
+        self._check(self.lib.kmcb200_smallk_write_db(self._h, path_prefix.encode(), cutoff_min, min(int(cutoff_max), (1 << 64) - 1),
+                                                     min(int(counter_max), (1 << 64) - 1), tot))
+        return tuple(int(x) for x in tot)
 
 
 def _as_u8(raw):

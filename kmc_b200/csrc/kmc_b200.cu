@@ -15,6 +15,7 @@
 #include "leaf_hash_wide.cuh"
 #include "split.cuh"
 #include "fastx.cuh"
+#include "small_k.cuh"
 
 #include <cmath>
 #include <cstddef>
@@ -1808,3 +1809,4 @@ int kmcb200_stage_names(kmcb200_ctx* ctx, uint32_t slot, char* buf, uint32_t cap
 #include "splitter.inl"
 #include "stage0.inl"
 #include "fastx.inl"
+#include "small_k.inl"

@@ -20,6 +20,11 @@ Parsing: by default (parse="host") every file is read whole and parsed in numpy 
 files are read in chunks of at most batch_bytes - 1 bytes into pinned host buffers by a reader thread, while the GPU parses
 (kmc_b200.FastxParser) and splits the previous chunk; the databases, totals and counts are the same.  A FASTQ / FASTA record must then fit
 in about half a chunk of raw bytes (the rest of a chunk after its last record end is carried into the next one).
+
+Small k (k <= 13, `count_reads_small_k`, `--small-k`): KMC's small-k mode.  Every k-mer is counted in a direct array of 4^k counters on the
+GPU (kmc_b200.SmallKCounter), with no bins, and the database is written in the KMC1 format the reference writes in that mode (version word
+0, no signature map), byte for byte `kmc -kK`'s when the reference takes its small-k path.  count_reads takes this path by itself where the
+bin path cannot run, k <= signature_len.
 """
 import argparse
 import json
@@ -32,8 +37,8 @@ import time
 
 import numpy as np
 
-from . import DbWriter, FASTA, FASTQ, FastxParser, KmcB200Error, ERR_INVALID, SignatureStats, Splitter, Stage2Context, Stage2Params, \
-    signature_map as _signature_map, stage2_bin_order
+from . import DbWriter, FASTA, FASTQ, FastxParser, KmcB200Error, ERR_INVALID, SignatureStats, SmallKCounter, Splitter, Stage2Context, \
+    Stage2Params, signature_map as _signature_map, stage2_bin_order
 
 _NL, _GT, _AT = 10, ord(">"), ord("@")
 STATS_SAMPLE_BYTES = 1 << 28                                            # STATS_FASTQ_SIZE (kmc_core/defs.h)
@@ -269,8 +274,59 @@ def signature_sample_counts(paths, k, signature_len, batch_bytes=1 << 26, device
     return counts
 
 
+SMALL_K_MAX = 13
+
+
+def count_reads_small_k(paths, out_prefix, k, cutoff_min=2, cutoff_max=1_000_000_000, counter_max=255, both_strands=True, batch_bytes=1 << 26,
+                        device=0, parse="host"):
+    """KMC's small-k mode (kmc_core/kmc.h:677-960) on one GPU, for 1 <= k <= 13: every batch of every file is counted into 4^k counters
+    (kmc_b200.SmallKCounter), then the KMC1 database is written (CSmallKCompleter::CompleteKMCFormat).  There are no bins: no signature
+    length, no map, and the LUT prefix length is the reference's choice for this mode, returned as `lut_prefix_len`.  parse as for
+    count_reads.  Returns the keys count_reads returns (n_super_kmers is 0, n_kmers equals n_total) plus lut_prefix_len."""
+    if parse not in ("host", "gpu"):
+        raise KmcB200Error(ERR_INVALID, "parse must be 'host' or 'gpu', not %r" % (parse,))
+    if not 1 <= k <= SMALL_K_MAX:
+        raise KmcB200Error(ERR_INVALID, "the small-k path counts k = 1..%d, not %d" % (SMALL_K_MAX, k))
+    t0 = time.perf_counter()
+    sk = SmallKCounter(k, both_strands, device, max_batch_bytes=batch_bytes)
+    n_bases = 0
+    read_s = 0.0
+    parsers = _Parsers(device, batch_bytes - 1) if parse == "gpu" else None
+    try:
+        for path in paths:
+            if parsers is not None:
+                with _RawChunks(path, batch_bytes - 1) as chunks:
+                    parser = None
+                    for chunk, final in chunks:
+                        parser = parser or parsers(chunk)
+                        chunks.consumed(sk.add_fastx(parser, chunk, final))
+                        n_bases += sk.last_seq_bytes
+                read_s += chunks.wait_s
+                continue
+            t = time.perf_counter()
+            with open(path, "rb") as f:
+                data = f.read()
+            read_s += time.perf_counter() - t
+            seq = sequences_to_batch(data)
+            del data
+            for batch in batches(seq, batch_bytes):
+                sk.add(batch)
+                n_bases += batch.size
+        t1 = time.perf_counter()
+        lp = sk.finish(cutoff_min, cutoff_max, counter_max)[0]
+        totals = sk.write_db(out_prefix, cutoff_min, cutoff_max, counter_max)
+    finally:
+        if parsers is not None:
+            parsers.close()
+        sk.close()
+    t2 = time.perf_counter()
+    return {"n_unique": totals[0], "n_cutoff_min": totals[1], "n_cutoff_max": totals[2], "n_total": totals[3], "n_super_kmers": 0,
+            "n_kmers": totals[3], "n_bases": n_bases, "stats_s": 0.0, "split_s": t1 - t0, "stage2_s": t2 - t1, "read_s": read_s,
+            "lut_prefix_len": lp}
+
+
 def count_reads(paths, out_prefix, k, signature_len, signature_map, lut_prefix_len, cutoff_min=2, cutoff_max=1_000_000_000, counter_max=255,
-                both_strands=True, batch_bytes=1 << 26, device=0, n_bins=None, parse="host"):
+                both_strands=True, batch_bytes=1 << 26, device=0, n_bins=None, parse="host", small_k=None):
     """KMC's stages on one GPU in RAM mode: every batch of every file is split on the GPU and the bin fragments stay in host memory;
     then bin by bin, stage 2 and the database writer.  Returns the writer's totals and the split's counts.
     With a signature_map: the bins are written in bin-id order, bin b's signatures (the map's preimage of b) go into .kmc_pre, and n_bins
@@ -279,9 +335,14 @@ def count_reads(paths, out_prefix, k, signature_len, signature_map, lut_prefix_l
     counts the (k+x)-mers of every bin, and the bins are written in the reference's stage-2 order (kmc_b200.stage2_bin_order); the map in
     .kmc_pre holds every signature's file position, 0 for the signatures that are not allowed.
     parse="host" reads every file whole and parses it in numpy; parse="gpu" reads chunks of batch_bytes - 1 bytes on a reader thread and
-    parses them on the GPU (kmc_b200.FastxParser, see the module docstring); the files and counts are the same either way."""
+    parses them on the GPU (kmc_b200.FastxParser, see the module docstring); the files and counts are the same either way.
+    small_k: None takes the small-k path (count_reads_small_k) where the bin path cannot run, k <= signature_len; True takes it for any
+    k <= 13, as `kmc` does; False keeps the bin path.  On the small-k path signature_len, signature_map, n_bins and lut_prefix_len are not
+    used, and the result also holds the lut_prefix_len the path chose."""
     if parse not in ("host", "gpu"):
         raise KmcB200Error(ERR_INVALID, "parse must be 'host' or 'gpu', not %r" % (parse,))
+    if small_k or (small_k is None and k <= signature_len):
+        return count_reads_small_k(paths, out_prefix, k, cutoff_min, cutoff_max, counter_max, both_strands, batch_bytes, device, parse)
     t0 = time.perf_counter()
     if signature_map is None:
         n_bins = DEFAULT_N_BINS if n_bins is None else int(n_bins)
@@ -388,20 +449,26 @@ def main(argv=None):
     ap.add_argument("--batch-bytes", type=int, default=1 << 26)
     ap.add_argument("--device", type=int, default=0)
     ap.add_argument("--gpu-parse", action="store_true", help="parse FASTQ / FASTA on the GPU in chunks of batch-bytes - 1 (default: numpy, whole files)")
+    ap.add_argument("--small-k", action="store_true",
+                    help="k <= 13: count in 4^k direct counters and write a KMC1 database, as kmc does (taken without the flag when k <= p)")
     a = ap.parse_args(argv)
     if len(a.inputs) < 2:
         ap.error("give at least one input and the output prefix")
+    parse = "gpu" if a.gpu_parse else "host"
     if a.map_from:
         m, sig_map = signature_map_from_kmc_pre(a.map_from)
     elif a.map:
         m, sig_map = a.signature_len, np.load(a.map)
     else:
         m, sig_map = a.signature_len, None
+    if a.small_k or a.k <= m:                                           # no bins: no map, and the path picks its own LUT prefix length
+        print(json.dumps(count_reads_small_k(a.inputs[:-1], a.inputs[-1], a.k, a.ci, a.cx, a.cs, not a.b, a.batch_bytes, a.device, parse)))
+        return 0
     lp = a.lut_prefix_len
     if lp is None:
         lp = next(p for p in (7, 3, 11, 15, 4, 5, 6, 2, 8, 9, 10, 12, 13, 14, 1) if p < a.k and (a.k - p) % 4 == 0)
     res = count_reads(a.inputs[:-1], a.inputs[-1], a.k, m, sig_map, lp, a.ci, a.cx, a.cs, not a.b, a.batch_bytes, a.device,
-                      a.n_bins if sig_map is None else None, parse="gpu" if a.gpu_parse else "host")
+                      a.n_bins if sig_map is None else None, parse=parse, small_k=False)
     print(json.dumps(res))
     return 0
 

@@ -67,6 +67,7 @@ struct ExpandArgs {
 	uint64_t* item_lo1;          // [total_tiles] first output record of the tile
 	uint16_t* item_cnt1;         // [total_tiles]
 	uint32_t top_shift;
+	const uint32_t* cell_scan;   // kExpandPartition: exclusive scan of cells1 = output index of (tile, digit) in recs
 	// oversized bins (kmc_b200.cu, run_oversized_bin): the bin is expanded chunk by chunk, once to count and once per key block
 	uint32_t mode;               // 0: everything (above); 1: only count the top 12 bits into hist12; 2: only k-mers of one key block, appended to recs
 	uint32_t fshift, fprefix, fmask;    // mode 2: keep the k-mers with ((kmer >> fshift) & fmask) == fprefix
@@ -77,7 +78,14 @@ struct ExpandArgs {
 	const uint64_t* region_start;        // [n_blocks] first record of every block's region inside recs
 	uint32_t n_blocks;                   // <= kExpandMaxBlocks
 };
-enum : uint32_t { kExpandAll = 0, kExpandCount12 = 1, kExpandFilter = 2, kExpandScatter = 3 };
+// kExpandCells + kExpandPartition: the bin path expands a bin of one-word records twice instead of writing the records in tile order and
+// partitioning them by their top digit afterwards.  kExpandCells only counts the level-1 digits of every tile into the cell layout; after
+// the cell scan, kExpandPartition extracts the k-mers again and writes each one to its level-1 bucket (the work of msd_partition_kernel,
+// with the extraction in place of the load).  The tile-ordered copy of the records (8N bytes written, 8N read back) never exists.
+enum : uint32_t { kExpandAll = 0, kExpandCount12 = 1, kExpandFilter = 2, kExpandScatter = 3, kExpandCells = 4, kExpandPartition = 5 };
+// kExpandPartition regroups a tile in shared memory over the staged bytes (8 bytes * 4096 records); wider records would need a larger
+// buffer than static shared memory allows and more registers for the keys it holds
+template <int WORDS> __host__ __device__ constexpr bool expand_partition_supported() { return WORDS == 1; }
 constexpr uint32_t kExpandMaxBlocks = 512;
 constexpr uint64_t kExpandUnknownRecs = ~0ull;      // n_rec of a chunk: not checked
 
@@ -522,19 +530,27 @@ __device__ __forceinline__ uint32_t msd_free_bits(const Rec<WORDS>& r, uint32_t 
 	return (uint32_t)v & mask;
 }
 
+// (<= 32 registers for one- and two-word records, <= 42 beyond: the occupancy the kernel was tuned at.  kExpandPartition holds the tile's
+// 8 k-mers and their ranks per thread across its barriers: <= 40 registers, 3 CTAs of 512 threads per SM, which measured faster than 2)
+template <int WORDS, uint32_t MODE>
+__host__ __device__ constexpr int expand_min_blocks() { return MODE == kExpandPartition ? 3 : WORDS <= 2 ? 2048 / ExpandCfg<WORDS>::kThreads : 6; }
+
 // MODE is a template parameter: the bin path (kExpandAll) must not pay registers / shared memory for the oversized-bin modes
 // (with the scatter code in the same instance the kernel needs more than 32 registers and the expansion is slower)
 template <int WORDS, uint32_t MODE = kExpandAll>
-__global__ void __launch_bounds__(ExpandCfg<WORDS>::kThreads, WORDS <= 2 ? 2048 / ExpandCfg<WORDS>::kThreads : 6) expand_kernel(const ExpandArgs a)      // (<= 32 registers for one- and two-word records, <= 42 beyond: the occupancy the kernel was tuned at)
+__global__ void __launch_bounds__(ExpandCfg<WORDS>::kThreads, expand_min_blocks<WORDS, MODE>()) expand_kernel(const ExpandArgs a)
 {
 	constexpr int kExpandTile = ExpandCfg<WORDS>::kTile, kExpandThreads = ExpandCfg<WORDS>::kThreads;
 	constexpr int IPT = kExpandTile / kExpandThreads;    // 8 k-mers per thread
 	constexpr int MAXSK = 1024, STAGE = 12288;          // per-tile staging of the super-k-mer index and bytes (typical tile: ~350 super-k-mers, ~4.5 KB)
 	constexpr int HW = kExpandTile / 32;                 // words of the head bitmap
+	// kExpandPartition regroups the tile's records in the staging buffer once they are all extracted
+	constexpr int SBYTES = MODE == kExpandPartition && kExpandTile * 8 * WORDS > STAGE + 32 ? kExpandTile * 8 * WORDS : STAGE + 32;
+	static_assert(MODE != kExpandPartition || expand_partition_supported<WORDS>(), "kExpandPartition: one-word records only");
 	__shared__ uint32_t hbits[HW];                       // bit s: a super-k-mer (other than the tile's first) starts at output slot s
 	__shared__ uint32_t hpre[HW];                        // set bits before the word
 	__shared__ uint32_t s_bit[MAXSK];                    // staged tiles: bit position of (k-mer of output slot 0) of every super-k-mer, minus 2 * slot
-	__shared__ __align__(16) uint8_t s_bytes[STAGE + 32];       // the tile's bytes as big-endian 32-bit words (+ slack: a funnel shift looks 2*WORDS words ahead)
+	__shared__ __align__(16) uint8_t s_bytes[SBYTES];    // the tile's bytes as big-endian 32-bit words (+ slack: a funnel shift looks 2*WORDS words ahead)
 	__shared__ uint32_t s_jmax;
 	__shared__ unsigned long long s_fbase;
 	__shared__ uint32_t warp_max[kExpandThreads / 32];   // (scratch of the filter mode)
@@ -543,11 +559,17 @@ __global__ void __launch_bounds__(ExpandCfg<WORDS>::kThreads, WORDS <= 2 ? 2048 
 	const uint32_t tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
 	const uint32_t le_mask = 0xffffffffu >> (31u - lane);
 	static_assert(kExpandThreads % 32 == 0, "output slot i * threads + tid belongs to lane tid % 32");
+	if constexpr (MODE == kExpandPartition)
+		if (a.flags[1] & kExpandAbortFlag) return;       // (a malformed bin also has no tiles)
 	if (tid < 256) htop[tid] = 0;
 	const uint32_t total_tiles = a.status[1];
 	Rec<WORDS>* __restrict__ out = reinterpret_cast<Rec<WORDS>*>(a.recs);
 
 	for (uint32_t g = blockIdx.x; g < total_tiles; g += gridDim.x) {
+		// kExpandPartition: output index of this tile's records of digit tid (cell tid * tiles + g), in flight during the tile's set-up
+		uint32_t digit_base = 0;
+		if constexpr (MODE == kExpandPartition)
+			if (tid < 256) digit_base = __ldg(a.cell_scan + g + (size_t)tid * total_tiles);
 		const uint4 da = __ldg(a.tile_desc + 2 * (size_t)g), db = __ldg(a.tile_desc + 2 * (size_t)g + 1);
 		if (g + gridDim.x < total_tiles) asm volatile("prefetch.global.L2 [%0];" ::"l"(a.tile_desc + 2 * (size_t)(g + gridDim.x)));
 		const uint64_t slot0 = da.x;
@@ -618,14 +640,30 @@ __global__ void __launch_bounds__(ExpandCfg<WORDS>::kThreads, WORDS <= 2 ? 2048 
 			return extract_kmer<WORDS>(a.bin + off[j] + 1, s, a.k, a.both_strands != 0,
 				[](uintptr_t wa) { return __ldg(reinterpret_cast<const unsigned long long*>(wa)); });
 		};
-		if constexpr (MODE == kExpandAll) {
+		// kExpandCells needs only the top digit of min(kmer, revcomp) = min(its first 4 symbols, the complement of its last 4 reversed):
+		// two 8-bit windows of the staged stream instead of the whole k-mer and its reverse complement (one-word records, k >= 4)
+		auto top_digit_of = [&](uint32_t slot) -> uint32_t {
+			if (WORDS > 1 || !staged || a.top_shift + 8u != 2u * a.k) return rec_top_digit<WORDS>(kmer_of(slot), a.top_shift);
+			const uint32_t rel = hpre[slot >> 5] + __popc(hbits[slot >> 5] & le_mask);
+			const uint32_t B = s_bit[rel] + 2u * slot;
+			const uint32_t* sw = reinterpret_cast<const uint32_t*>(s_bytes);
+			auto byte_at = [&](uint32_t b) { const uint32_t wi = b >> 5; return __funnelshift_l(sw[wi + 1], sw[wi], b & 31u) >> 24; };
+			const uint32_t f = byte_at(B);
+			if (!a.both_strands) return f;
+			uint32_t r = ~byte_at(B + 2u * a.k - 8u) & 0xFFu;
+			r = ((r & 0x03u) << 6) | ((r & 0x0Cu) << 2) | ((r & 0x30u) >> 2) | ((r & 0xC0u) >> 6);
+			return min(f, r);
+		};
+		if constexpr (MODE == kExpandAll || MODE == kExpandCells) {
 #pragma unroll kExpandUnroll
 			for (int i = 0; i < IPT; ++i) {
 				const uint32_t slot = i * kExpandThreads + tid;
 				if (slot < cnt) {
-					const Rec<WORDS> r = kmer_of(slot);
-					out[obase + slot] = r;
-					atomicAdd(&htop[rec_top_digit<WORDS>(r, a.top_shift)], 1u);
+					if constexpr (MODE == kExpandAll) {
+						const Rec<WORDS> r = kmer_of(slot);
+						out[obase + slot] = r;
+						atomicAdd(&htop[rec_top_digit<WORDS>(r, a.top_shift)], 1u);
+					} else atomicAdd(&htop[top_digit_of(slot)], 1u);          // (counts only: kExpandPartition writes the records)
 				}
 			}
 			__syncthreads();
@@ -635,6 +673,59 @@ __global__ void __launch_bounds__(ExpandCfg<WORDS>::kThreads, WORDS <= 2 ? 2048 
 				htop[tid] = 0;
 			}
 			if (tid == 0) { a.item_lo1[g] = obase; a.item_cnt1[g] = (uint16_t)cnt; }
+		} else if constexpr (MODE == kExpandPartition) {
+			// level-1 partition of the tile straight from the bin (msd_partition_kernel's consumer, with the extraction in place of the load):
+			// rank inside (tile, digit) = return value of one shared-memory atomicAdd, scan of the digit counts, regroup by digit in shared
+			// memory, digit-contiguous runs leave with coalesced stores
+			__shared__ uint32_t s_excl[256], s_goff[256];
+			Rec<WORDS> key[IPT];
+			uint32_t rank[IPT / 2] = {};          // two 16-bit ranks per register (a tile holds at most 4096 records)
+#pragma unroll
+			for (int i = 0; i < IPT; ++i) {
+				const uint32_t slot = i * kExpandThreads + tid;
+				if (slot < cnt) {
+					key[i] = kmer_of(slot);
+					rank[i / 2] |= atomicAdd(&htop[rec_top_digit<WORDS>(key[i], a.top_shift)], 1u) << (16 * (i & 1));
+				}
+			}
+			__syncthreads();
+			uint32_t c = 0, inc = 0;
+			if (tid < 256) {          // (warps 0..7; every thread zeroes its own digit for the next tile)
+				c = htop[tid];
+				htop[tid] = 0;
+				inc = c;
+#pragma unroll
+				for (int o = 1; o < 32; o <<= 1) {
+					const uint32_t x = __shfl_up_sync(0xffffffffu, inc, o);
+					if (lane >= (uint32_t)o) inc += x;
+				}
+				if (lane == 31) warp_max[warp] = inc;
+			}
+			__syncthreads();
+			if (tid < 256) {
+				uint32_t ex = inc - c;
+#pragma unroll
+				for (int w = 0; w < 8; ++w) if ((uint32_t)w < warp) ex += warp_max[w];
+				s_excl[tid] = ex;
+				s_goff[tid] = digit_base - ex;          // global index of tile-sorted position q is s_goff[d] + q
+			}
+			__syncthreads();
+			// every k-mer of the tile is in registers: the staged bytes are free for the regrouping (the next tile stages after a barrier)
+			Rec<WORDS>* buf = reinterpret_cast<Rec<WORDS>*>(s_bytes);
+#pragma unroll
+			for (int i = 0; i < IPT; ++i) {
+				const uint32_t slot = i * kExpandThreads + tid;
+				if (slot < cnt) buf[s_excl[rec_top_digit<WORDS>(key[i], a.top_shift)] + ((rank[i / 2] >> (16 * (i & 1))) & 0xFFFFu)] = key[i];
+			}
+			__syncthreads();
+#pragma unroll
+			for (int i = 0; i < IPT; ++i) {
+				const uint32_t q = i * kExpandThreads + tid;
+				if (q < cnt) {
+					const Rec<WORDS> r = buf[q];
+					out[s_goff[rec_top_digit<WORDS>(r, a.top_shift)] + q] = r;
+				}
+			}
 		} else if constexpr (MODE == kExpandCount12) {
 			// oversized bin, first pass: where do the k-mers fall?  (top 12 bits; nothing is written)
 			for (int i = 0; i < IPT; ++i) {

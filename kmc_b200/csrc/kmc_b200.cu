@@ -43,7 +43,10 @@ constexpr uint32_t kHeavyListCap = 2048;           // leaves of more than kLwHea
 
 thread_local std::string g_create_error;
 
-enum { kHistNone = 0, kHistTiles = 1, kHistAligned = 2 };      // level-1 cells: none yet / per expand tile (expand.cuh) / per aligned tile (expand_fused.cuh)
+// level-1 cells: none yet / per expand tile (expand.cuh) / per aligned tile (expand_fused.cuh) / per expand tile, and the records are not
+// written yet: the level-1 partition expands the bin a second time (expand_kernel<kExpandPartition>) with the arguments kept in
+// Slot::expand_args
+enum { kHistNone = 0, kHistTiles = 1, kHistAligned = 2, kHistCells = 3 };
 
 struct ZeroBlock {                                // zeroed with one memset at the start of every bin
 	uint64_t hist[kHistRows][256];
@@ -98,7 +101,8 @@ struct Slot {
 	uint32_t last_n_packs = 1;
 	uint64_t* cdesc = nullptr; size_t cdesc_cap = 0;        // count look-back descriptors
 	uint64_t* pdesc = nullptr; size_t pdesc_cap = 0;        // pack look-back descriptors of the fused expansion
-	int hist_mode = 0;                                      // what the last expansion left for the sort: kHistNone / kHistTiles / kHistAligned
+	int hist_mode = 0;                                      // what the last expansion left for the sort: kHistNone / kHistTiles / kHistAligned / kHistCells
+	ExpandArgs expand_args{};                               // kHistCells: the counting expansion's arguments, for the level-1 partition
 	// outputs of the host-buffer path
 	uint8_t* d_out = nullptr; size_t out_cap = 0;
 	uint64_t* d_lut = nullptr;
@@ -130,7 +134,7 @@ struct kmcb200_ctx {
 	uint32_t key_bytes = 0, suffix_bytes = 0, counter_bytes = 0;
 	uint64_t lut_entries = 0;
 	int sm_count = 0;
-	int occ_radix = 1, occ_expand = 1, occ_msd_part = 1, occ_msd_part_wide = 1, occ_msd_local = 1;
+	int occ_radix = 1, occ_expand = 1, occ_expand_part = 1, occ_msd_part = 1, occ_msd_part_wide = 1, occ_msd_local = 1;
 	uint32_t force_b2 = 0;                                  // KMCB200_L2_BITS: bits of the second partition level (0: chosen from the bin size)
 	bool use_msd = true;                                    // KMCB200_SORT=lsd forces the plain 8-bit LSD passes
 	bool use_fused = false;                                 // KMCB200_EXPAND=fused: the single-pass expansion (expand_fused.cuh) - measured slower than the index-based kernels, kept as an option
@@ -259,6 +263,8 @@ int setup_kernels(kmcb200_ctx* ctx)
 	CU(cudaFuncSetAttribute(lsd_sort_kernel<WORDS>, cudaFuncAttributeMaxDynamicSharedMemorySize, SortSmem<WORDS>::kBytes));
 	CU(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&ctx->occ_radix, lsd_sort_kernel<WORDS>, SortCfg<WORDS>::kThreads, SortSmem<WORDS>::kBytes));
 	CU(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&ctx->occ_expand, expand_kernel<WORDS>, ExpandCfg<WORDS>::kThreads, 0));
+	if constexpr (expand_partition_supported<WORDS>())
+		CU((cudaOccupancyMaxActiveBlocksPerMultiprocessor(&ctx->occ_expand_part, expand_kernel<WORDS, kExpandPartition>, ExpandCfg<WORDS>::kThreads, 0)));
 	CU(cudaFuncSetAttribute(expand_fused_kernel<WORDS>, cudaFuncAttributeMaxDynamicSharedMemorySize, FxSmem<WORDS>::kBytes));
 	const size_t cs = count_smem_bytes<WORDS>(ctx->suffix_bytes + ctx->counter_bytes);
 	CU(cudaFuncSetAttribute(count_emit_kernel<WORDS>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)cs));
@@ -282,9 +288,16 @@ int launch_expand(kmcb200_ctx* ctx, const ExpandArgs& a, cudaStream_t st)
 {
 	const uint64_t n_bound = a.n_rec == kExpandUnknownRecs ? a.size * 4 : a.n_rec;
 	const uint32_t max_tiles = (uint32_t)(n_bound / ExpandCfg<WORDS>::kTile) + a.n_packs + 1;
-	const uint32_t grid = std::min<uint32_t>(max_tiles, (uint32_t)(ctx->sm_count * ctx->occ_expand));
+	const uint32_t grid = std::min<uint32_t>(max_tiles, (uint32_t)(ctx->sm_count * (a.mode == kExpandPartition ? std::max(ctx->occ_expand_part, 1) : ctx->occ_expand)));
 	switch (a.mode) {
 	case kExpandAll: expand_kernel<WORDS, kExpandAll><<<grid, ExpandCfg<WORDS>::kThreads, 0, st>>>(a); break;
+	case kExpandCells:
+	case kExpandPartition:
+		if constexpr (expand_partition_supported<WORDS>()) {
+			if (a.mode == kExpandCells) expand_kernel<WORDS, kExpandCells><<<grid, ExpandCfg<WORDS>::kThreads, 0, st>>>(a);
+			else expand_kernel<WORDS, kExpandPartition><<<grid, ExpandCfg<WORDS>::kThreads, 0, st>>>(a);
+			break;
+		} else return fail(ctx, KMCB200_ERR_INVALID, "no level-1 partition expansion for %d-word records", WORDS);
 	case kExpandCount12: expand_kernel<WORDS, kExpandCount12><<<grid, ExpandCfg<WORDS>::kThreads, 0, st>>>(a); break;
 	case kExpandScatter: expand_kernel<WORDS, kExpandScatter><<<grid, ExpandCfg<WORDS>::kThreads, 0, st>>>(a); break;
 	default: expand_kernel<WORDS, kExpandFilter><<<grid, ExpandCfg<WORDS>::kThreads, 0, st>>>(a); break;
@@ -386,8 +399,12 @@ struct LeafPlan {
 	uint32_t n_leaves = 0, low_bits = 0;
 };
 
+// launch_sort takes the hybrid MSD path (else: the LSD passes alone) for n records with key_bits significant bits
+bool msd_path(const kmcb200_ctx* ctx, uint64_t n, uint32_t key_bits) { return ctx->use_msd && key_bits >= 24 && n >= (1u << 16); }
+
 // Sorts n records from `a` (with `b` as the second buffer).  *result_in_b tells where the sorted records end up.
 // hist_ready: the expand stage has zeroed the slot's ZeroBlock and written the level-1 cells / items.
+// kHistCells: ... and `a` holds no records yet: the level-1 partition expands them from the bin into `b` (MSD path only).
 template <int WORDS>
 int launch_sort(kmcb200_ctx* ctx, Slot& s, void* a, void* b, uint64_t n, uint32_t key_bytes, uint32_t key_bits, int hist_mode, uint32_t n_packs, cudaStream_t st, bool* result_in_b, LeafPlan* plan = nullptr)
 {
@@ -397,12 +414,13 @@ int launch_sort(kmcb200_ctx* ctx, Slot& s, void* a, void* b, uint64_t n, uint32_
 	if (n_tiles64 > 0x7fffffffull || n >= (1ull << 32)) return fail(ctx, KMCB200_ERR_INVALID, "bin too large: %llu records", (unsigned long long)n);
 	const uint32_t n_tiles = (uint32_t)n_tiles64;
 	// key_bits: significant bits of a record.  2k for records we expanded ourselves; all key bytes for foreign records (seam #1)
-	const bool msd = ctx->use_msd && key_bits >= 24 && n >= (1u << 16);
+	const bool msd = msd_path(ctx, n, key_bits);
+	if (hist_mode == kHistCells && !msd) return fail(ctx, KMCB200_ERR_INVALID, "the records of this bin were not expanded");
 	const uint32_t top_shift = key_bits - 8;
 	if (int rc = ensure(ctx, s.desc, s.desc_cap, (size_t)n_tiles * 256, true)) return rc;
 	if (msd) if (int rc = ensure_msd<WORDS>(ctx, s, n, n_packs, choose_nd2<WORDS>(ctx, n, plan != nullptr))) return rc;      // (sized alike by stage_expand: no reallocation here when its cells are in use)
 
-	const bool hist_ready = hist_mode == kHistTiles;
+	const bool hist_ready = hist_mode == kHistTiles || hist_mode == kHistCells;
 	if (hist_mode == kHistNone) if (int rc = zero_async(ctx, s.zero, sizeof(ZeroBlock), st)) return rc;
 	int iv = 0;      // timed interval index
 	CU(cudaEventRecord(s.ev_pass[0], st));
@@ -424,7 +442,7 @@ int launch_sort(kmcb200_ctx* ctx, Slot& s, void* a, void* b, uint64_t n, uint32_
 		const int local_smem = msd_local_cap<WORDS>() * 8 * WORDS + (MsdLocalCfg<WORDS>::kThreads / 32) * 1024;
 
 		MsdItems items1{};
-		if (hist_ready) {          // items and cells were written by expand_kernel
+		if (hist_ready) {          // items and cells were written by expand_kernel (kExpandAll / kExpandCells)
 			items1.item_lo = s.msd_item_lo1; items1.item_cnt = s.msd_item_cnt1; items1.n_items = &s.zero->status[1];
 		} else if (hist_mode == kHistAligned) {          // the fused expansion counted per aligned tile; its init kernel wrote the one-segment item tables
 			items1.seg_start = s.msd_seg1; items1.item_base = s.msd_item_base1; items1.item_seg = s.msd_item_seg2; items1.n_items = s.msd_item_base1 + 1;
@@ -447,10 +465,19 @@ int launch_sort(kmcb200_ctx* ctx, Slot& s, void* a, void* b, uint64_t n, uint32_
 		p1.in = a; p1.out = b; p1.items = items1; p1.cell_scan = s.msd_cell_scan; p1.shift = top_shift; p1.nd = 256;
 		p1.flags = never;
 		// (the item_seg table of the level-2 items shares its buffer with the all-zero level-1 table: partition first, bounds after)
-		msd_partition_kernel<WORDS><<<pgrid1, MsdCfg<WORDS>::kThreads + 32, MsdSmem<WORDS>::kBytes, st>>>(p1);
-		s.pass_names[iv] = "msd_partition_L1"; CU(cudaEventRecord(s.ev_pass[++iv], st));
+		if (hist_mode == kHistCells) {          // the records go from the bin straight into their level-1 buckets in b
+			ExpandArgs ea = s.expand_args;
+			ea.mode = kExpandPartition; ea.recs = b; ea.cell_scan = s.msd_cell_scan;
+			if (int rc = launch_expand<WORDS>(ctx, ea, st)) return rc;
+			s.pass_names[iv] = "expand_scatter_L1";
+		} else {
+			msd_partition_kernel<WORDS><<<pgrid1, MsdCfg<WORDS>::kThreads + 32, MsdSmem<WORDS>::kBytes, st>>>(p1);
+			ctx->launches++;
+			s.pass_names[iv] = "msd_partition_L1";
+		}
+		CU(cudaEventRecord(s.ev_pass[++iv], st));
 		msd_bounds_kernel<<<1, 1024, 0, st>>>(b1);
-		ctx->launches += 2;
+		ctx->launches++;
 		if (b2 > 0) {
 			MsdItems items2{};
 			items2.seg_start = s.msd_start2; items2.item_base = s.msd_item_base2; items2.item_seg = s.msd_item_seg2; items2.n_items = &s.zero->msd_n_items[1];
@@ -646,7 +673,8 @@ int stage_expand(kmcb200_ctx* ctx, Slot& s, const uint8_t* d_bin, uint64_t size,
 		s.hist_mode = kHistAligned;
 		return 0;
 	}
-	s.hist_mode = em.mode == kExpandAll ? kHistTiles : kHistNone;
+	const bool cells = em.mode == kExpandAll || em.mode == kExpandCells;          // the expansion writes the level-1 cells
+	s.hist_mode = em.mode == kExpandAll ? kHistTiles : em.mode == kExpandCells ? kHistCells : kHistNone;
 
 	if (int rc = ensure(ctx, s.sk_off, s.sk_off_cap, size / min_rec + 2)) return rc;
 	if (int rc = ensure(ctx, s.sk_kpre, s.sk_kpre_cap, size / min_rec + 2)) return rc;
@@ -666,15 +694,17 @@ int stage_expand(kmcb200_ctx* ctx, Slot& s, const uint8_t* d_bin, uint64_t size,
 	a.recs = d_recs;
 	a.mode = em.mode; a.fshift = em.fshift; a.fprefix = em.fprefix; a.fmask = em.fmask; a.hist12 = em.hist12; a.out_counter = em.out_counter;
 	a.blk_of_prefix = em.blk_of_prefix; a.region_start = em.region_start; a.n_blocks = em.n_blocks;
-	if (em.mode == kExpandAll) {
+	if (cells) {
 		if (int rc = DISPATCH_WORDS(ctx, ensure_msd, ctx, s, n_rec, np, DISPATCH_WORDS(ctx, choose_nd2, ctx, n_rec, ctx->use_leaf))) return rc;
 		a.cells1 = s.msd_cells; a.item_lo1 = s.msd_item_lo1; a.item_cnt1 = s.msd_item_cnt1;
 	} else { a.cells1 = nullptr; a.item_lo1 = nullptr; a.item_cnt1 = nullptr; }
 	a.top_shift = std::max(2u * k, 8u) - 8u;
+	a.cell_scan = nullptr;
+	if (em.mode == kExpandCells) s.expand_args = a;
 
 	bin_init_kernel<<<64, 256, 0, st>>>(reinterpret_cast<uint32_t*>(s.zero), (uint32_t)(sizeof(ZeroBlock) / 4), reinterpret_cast<uint32_t*>(zero_lut),
 		(size_t)ctx->lut_entries * 2, reinterpret_cast<uint32_t*>(zero_result), InitExtra());
-	if (s.have_extras && em.mode == kExpandAll) {          // N4: stage 1 handed over the length bytes: two prefix sums per pack instead of the walk
+	if (s.have_extras && cells) {          // N4: stage 1 handed over the length bytes: two prefix sums per pack instead of the walk
 		index_from_extras_kernel<<<np, 1024, 0, st>>>(a, s.d_extras, s.d_pack_rec);
 		ctx->launches += 2;
 		big_pack = false;
@@ -915,7 +945,11 @@ int run_bin(kmcb200_ctx* ctx, Slot& s, const uint8_t* d_bin, uint64_t size, uint
 	}
 	if (int rc = ensure(ctx, s.recs_a, s.recs_a_cap, n_rec * rec_bytes)) return rc;
 	if (int rc = ensure(ctx, s.recs_b, s.recs_b_cap, n_rec * rec_bytes)) return rc;
-	if (int rc = stage_expand(ctx, s, d_bin, size, n_rec, pack_bytes, n_packs, s.recs_a, st, ExpandMode(), packs_uploaded, d_lut, d_result, st_walk)) return rc;
+	// a bin of one-word records that takes the MSD path is expanded twice, once to count the level-1 digits, once into the level-1 buckets
+	// (expand.cuh, kExpandCells / kExpandPartition): its records are never written in tile order and read back by a separate partition pass
+	ExpandMode em;
+	if (expand_partition_supported<1>() && ctx->words == 1 && !ctx->use_fused && n_rec < (1ull << 32) && msd_path(ctx, n_rec, 2u * ctx->prm.kmer_len)) em.mode = kExpandCells;
+	if (int rc = stage_expand(ctx, s, d_bin, size, n_rec, pack_bytes, n_packs, s.recs_a, st, em, packs_uploaded, d_lut, d_result, st_walk)) return rc;
 	CU(cudaEventRecord(s.ev_expand, st));
 	s.ran_expand = true;
 	bool in_b = false;

@@ -1,9 +1,10 @@
-import os, sys
 """Development probe: time of the index + expand stage alone (kmcb200_dev_expand) for the library named by KMCB200_LIB."""
 import os, sys
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
+sys.path.insert(0, os.path.join(ROOT, "tests"))
 import torch, kmc_b200
+from kmc_testlib import fast_bin
 n_rec = 1 << 26
 dev = torch.device("cuda", 0)
 hb = fast_bin(1000, 31, n_rec)

@@ -1,9 +1,10 @@
-import os, sys
 """Development probe: per-stage / per-pass CUDA-event times of one resident bin (k=31, 2^26 k-mers by default)."""
 import sys, os
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
+sys.path.insert(0, os.path.join(ROOT, "tests"))
 import numpy as np, torch, kmc_b200
+from kmc_testlib import fast_bin
 
 n_rec = int(sys.argv[1]) if len(sys.argv) > 1 else 1 << 26
 k = int(sys.argv[2]) if len(sys.argv) > 2 else 31

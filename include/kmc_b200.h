@@ -22,18 +22,15 @@
  *   KMCB200_SORT=lsd               plain 8-bit LSD passes instead of the hybrid MSD sort
  *   KMCB200_LEAF=sort              sort the leaves on chip + count_emit instead of counting them in hash tables
  *   KMCB200_LEAF_SLOT_BITS=8|9|10  slots of a warp's leaf table (default 10; not leaf_hash_cta_kernel's: KMCB200_LEAF_CTA)
- *   KMCB200_LEAF_KERNEL=cta|hash|warp  one-word records always by one table per CTA (leaf_hash_cta_kernel) / one table per warp (leaf_hash_kernel) /
- *                                  round 1's leaf kernel (ordered groups, leaf_warp.cuh); default: the CTA kernel in bins whose mean leaf is > 1280
- *                                  records, leaf_hash_kernel below; KMCB200_LEAF_WIDE=warp: round 1's kernel for records of > 1 word
- *   KMCB200_LEAF_CTA=W:B           leaf_hash_cta_kernel: W warps per CTA share one table of 2^B slots; 4:12 (default), 8:12, 8:13 or 4:10
+ *   KMCB200_LEAF_KERNEL=cta|hash   one-word records always by one table per CTA (leaf_hash_cta_kernel) / one table per warp (leaf_hash_kernel);
+ *                                  default: the CTA kernel in bins whose mean leaf is > 1280 records, leaf_hash_kernel below
+ *   KMCB200_LEAF_CTA=4:B           leaf_hash_cta_kernel: 4 warps per CTA share one table of 2^B slots; 4:12 (default) or 4:10
  *   KMCB200_LEAF_FILL_PCT=n        the hash kernels plan a table round for this load (default 62); KMCB200_LEAF_RATIO0=n: first guess of distinct k-mers per record x 256 (default 90)
- *   KMCB200_LEAF_ROUND_PCT=n       leaf_warp_kernel: records per table round in percent of the slots (default 100)
  *   KMCB200_L2_BITS=1..10          bits of the second partition level (default: from the bin size: 8 for one-word records; wider records up to 10)
  *   KMCB200_LEAF_TARGET=n, KMCB200_LEAF_MAX_B2=8..10   mean leaf size / most bits the default rule aims at for one-word records (1024, 8)
  *   KMCB200_MAX_BLOCK_RECORDS=n    a bin with more k-mers is counted key block by key block (default: what 60 % of the free HBM holds, < 2^32)
  *   KMCB200_KEY_BLOCKS=filter     key blocks of an oversized bin re-expand it with a filter (default: one scattering expansion when the records fit in HBM once)
  *   KMCB200_KEY_BLOCK_RECORDS=n    preferred size of a key block in the scattering flow (default 2^28)
- *   KMCB200_EXPAND=fused           single-pass expansion (expand_fused.cuh) instead of the index-based kernels (measured slower; option)
  *   KMCB200_OVERLAP_WALK=0         index kernels of a submitted bin on the compute stream instead of its copy stream
  *   KMCB200_MAX_CHUNK_BYTES=n      ... and expanded in chunks of at most n bytes (default 2^30)
  */

@@ -1,11 +1,11 @@
 // kmc_b200 — host side of the C ABI (include/kmc_b200.h): context, HBM workspace, launch sequences.
 // The per-bin sequence mirrors CKmerBinSorter<SIZE>::ProcessBins (kmc_core/kb_sorter.h:210-237):
-//   Expand (index + expand kernels) -> Sort (two MSD partition levels) + Compact fused in the leaf kernels (leaf_hash.cuh, leaf_hash_wide.cuh);
+//   Expand (index + expand kernels) -> Sort (two MSD partition levels) + Compact fused in the leaf kernels (leaf_hash_cta.cuh, leaf_hash.cuh,
+//   leaf_hash_wide.cuh; one-word leaves with a dominant k-mer: leaf_warp.cuh);
 //   behind a device flag: Sort (one cooperative lsd_sort_kernel over all key bytes) -> Compact (count_emit_kernel).
 #include "../../include/kmc_b200.h"
 #include "common.cuh"
 #include "expand.cuh"
-#include "expand_fused.cuh"
 #include "radix_sort.cuh"
 #include "count.cuh"
 #include "msd_sort.cuh"
@@ -43,10 +43,9 @@ constexpr uint32_t kHeavyListCap = 2048;           // leaves of more than kLwHea
 
 thread_local std::string g_create_error;
 
-// level-1 cells: none yet / per expand tile (expand.cuh) / per aligned tile (expand_fused.cuh) / per expand tile, and the records are not
-// written yet: the level-1 partition expands the bin a second time (expand_kernel<kExpandPartition>) with the arguments kept in
-// Slot::expand_args
-enum { kHistNone = 0, kHistTiles = 1, kHistAligned = 2, kHistCells = 3 };
+// level-1 cells: none yet / per expand tile (expand.cuh) / per expand tile, and the records are not written yet: the level-1 partition
+// expands the bin a second time (expand_kernel<kExpandPartition>) with the arguments kept in Slot::expand_args
+enum { kHistNone = 0, kHistTiles = 1, kHistCells = 2 };
 
 struct ZeroBlock {                                // zeroed with one memset at the start of every bin
 	uint64_t hist[kHistRows][256];
@@ -55,7 +54,6 @@ struct ZeroBlock {                                // zeroed with one memset at t
 	uint32_t msd_flags[4];                        // [0] kMsdFlagFallback (leaves too large -> LSD passes), [1] always 0
 	uint32_t msd_n_items[2];                      // work items of the level-1 / level-2 segmentation
 	uint32_t msd_counters[4];                     // tickets: level-1 partition, level-2 partition, leaves, leaf-count
-	uint32_t pack_ticket[4];                      // fused expansion: packs are taken in order
 	uint32_t heavy_count[2];                      // [0] large leaves noted by the leaf kernel, [1] ticket of the second (HEAVY) launch
 	uint32_t heavy_list[kHeavyListCap];           // their leaf ids
 	uint32_t leaf_group_sum[kMaxLeaves / 1024];   // emitted records per group of 1024 leaves
@@ -100,8 +98,7 @@ struct Slot {
 	const char* pass_names[kMaxPasses + 8] = {};
 	uint32_t last_n_packs = 1;
 	uint64_t* cdesc = nullptr; size_t cdesc_cap = 0;        // count look-back descriptors
-	uint64_t* pdesc = nullptr; size_t pdesc_cap = 0;        // pack look-back descriptors of the fused expansion
-	int hist_mode = 0;                                      // what the last expansion left for the sort: kHistNone / kHistTiles / kHistAligned / kHistCells
+	int hist_mode = 0;                                      // what the last expansion left for the sort: kHistNone / kHistTiles / kHistCells
 	ExpandArgs expand_args{};                               // kHistCells: the counting expansion's arguments, for the level-1 partition
 	// outputs of the host-buffer path
 	uint8_t* d_out = nullptr; size_t out_cap = 0;
@@ -137,18 +134,14 @@ struct kmcb200_ctx {
 	int occ_radix = 1, occ_expand = 1, occ_expand_part = 1, occ_msd_part = 1, occ_msd_part_wide = 1, occ_msd_local = 1;
 	uint32_t force_b2 = 0;                                  // KMCB200_L2_BITS: bits of the second partition level (0: chosen from the bin size)
 	bool use_msd = true;                                    // KMCB200_SORT=lsd forces the plain 8-bit LSD passes
-	bool use_fused = false;                                 // KMCB200_EXPAND=fused: the single-pass expansion (expand_fused.cuh) - measured slower than the index-based kernels, kept as an option
 	bool scatter_blocks = true;                             // KMCB200_KEY_BLOCKS=filter: key blocks always re-expand the bin with a filter (what happens anyway when the records do not fit in HBM once)
 	uint64_t key_block_records = 1ull << 28;                // KMCB200_KEY_BLOCK_RECORDS: preferred size of a key block when the bin is scattered once (leaves of ~1-2 K records)
 	bool overlap_walk = true;                               // KMCB200_OVERLAP_WALK=0: the index kernels of a submitted bin on the compute stream instead of its copy stream
 	bool use_leaf = true;                                   // KMCB200_LEAF=sort sorts the leaves + count_emit instead of counting them
-	int occ_leaf = 1;
 	int occ_leaf_hash = 1;
-	bool leaf_hash_wide = true;                             // KMCB200_LEAF_WIDE = hash | warp: records of more than one word by leaf_hash_wide_kernel / leaf_warp_kernel
-	bool leaf_hash = true;                                  // KMCB200_LEAF_KERNEL = hash | warp: one-word records are counted by leaf_hash_kernel (round 2) / leaf_warp_kernel
 	int leaf_cta = 2;                                       // one-word records by leaf_hash_cta_kernel (one table per CTA): 2 = in bins of mean leaves > kLeafCtaMinMean,
-	                                                        // 1 = always (KMCB200_LEAF_KERNEL=cta), 0 = never (KMCB200_LEAF_KERNEL = hash | warp)
-	int leaf_cta_warps = 4, leaf_cta_slot_bits = 12;        // KMCB200_LEAF_CTA = W:B, its warps per CTA and table slots (2^B)
+	                                                        // 1 = always (KMCB200_LEAF_KERNEL=cta), 0 = never (KMCB200_LEAF_KERNEL=hash: leaf_hash_kernel)
+	int leaf_cta_slot_bits = 12;                            // KMCB200_LEAF_CTA = 4:B, the 2^B slots of leaf_hash_cta_kernel's table (4 warps per CTA)
 	int occ_leaf_cta = 1;
 	uint32_t leaf_max_b2 = 8;                               // KMCB200_LEAF_MAX_B2 (8: on the H100 the 512 / 1024-digit level 2 costs more than it saves, DESIGN 3.1)
 	uint32_t leaf_target = 1024;                            // KMCB200_LEAF_TARGET: mean leaf size the second partition level of a large bin aims at (leaf_hash_kernel)
@@ -156,7 +149,6 @@ struct kmcb200_ctx {
 	uint32_t leaf_ratio0_q8 = 90;                           // KMCB200_LEAF_RATIO0: first guess of distinct k-mers per record, x 256 (30x coverage, 1 % errors: ~0.3)
 	uint64_t max_block_records = 1ull << 28;                // a bin with more k-mers is counted key block by key block: from the free HBM at create (KMCB200_MAX_BLOCK_RECORDS overrides)
 	uint64_t max_chunk_bytes = 1ull << 30;                  // KMCB200_MAX_CHUNK_BYTES: ... and expanded chunk by chunk
-	uint32_t leaf_round_pct = 100;                          // KMCB200_LEAF_ROUND_PCT: records per table round in percent of the slots
 	int leaf_slot_bits = 10;                                // KMCB200_LEAF_SLOT_BITS = 8 | 9 | 10: slots of a warp's leaf table
 	uint32_t epoch = 1;
 	uint64_t launches = 0;
@@ -206,20 +198,12 @@ int zero_async(kmcb200_ctx* ctx, void* ptr, size_t bytes, cudaStream_t st)
 }
 
 // start of a bin: the slot's ZeroBlock, and (when given) the LUT and the 8 result words, in ONE launch
-struct InitExtra {            // the fused expansion (expand_fused.cuh): zeroed level-1 cells, the level-1 items are the aligned tiles of [0, n)
-	uint32_t* cells = nullptr; size_t cell_words = 0;
-	uint32_t* item_seg = nullptr; size_t item_seg_words = 0;
-	uint64_t* seg1 = nullptr; uint32_t* item_base1 = nullptr; uint64_t n = 0; uint32_t n_tiles = 0;
-};
-__global__ void bin_init_kernel(uint32_t* zero_block, uint32_t zero_words, uint32_t* lut, size_t lut_words, uint32_t* result, const InitExtra x)
+__global__ void bin_init_kernel(uint32_t* zero_block, uint32_t zero_words, uint32_t* lut, size_t lut_words, uint32_t* result)
 {
 	const size_t stride = (size_t)gridDim.x * blockDim.x, i0 = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
 	for (size_t i = i0; i < zero_words; i += stride) zero_block[i] = 0u;
 	if (lut) for (size_t i = i0; i < lut_words; i += stride) lut[i] = 0u;
 	if (result && i0 < 16) result[i0] = 0u;
-	if (x.cells) for (size_t i = i0; i < x.cell_words; i += stride) x.cells[i] = 0u;
-	if (x.item_seg) for (size_t i = i0; i < x.item_seg_words; i += stride) x.item_seg[i] = 0u;
-	if (x.seg1 && i0 == 0) { x.seg1[0] = 0; x.seg1[1] = x.n; x.item_base1[0] = 0; x.item_base1[1] = x.n_tiles; }
 }
 
 uint32_t byte_log(uint64_t x) { return x < (1u << 8) ? 1 : x < (1u << 16) ? 2 : x < (1u << 24) ? 3 : 4; }   // defs.h:121
@@ -245,7 +229,6 @@ int next_epoch(kmcb200_ctx* ctx, uint32_t* out, uint32_t count = 1)
 		for (auto& s : ctx->slots) {
 			if (s.desc) CU(cudaMemset(s.desc, 0, s.desc_cap * sizeof(uint64_t)));
 			if (s.cdesc) CU(cudaMemset(s.cdesc, 0, s.cdesc_cap * sizeof(uint64_t)));
-			if (s.pdesc) CU(cudaMemset(s.pdesc, 0, s.pdesc_cap * sizeof(uint64_t)));
 		}
 		CU(cudaDeviceSynchronize());
 		ctx->epoch = 1;
@@ -265,7 +248,6 @@ int setup_kernels(kmcb200_ctx* ctx)
 	CU(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&ctx->occ_expand, expand_kernel<WORDS>, ExpandCfg<WORDS>::kThreads, 0));
 	if constexpr (expand_partition_supported<WORDS>())
 		CU((cudaOccupancyMaxActiveBlocksPerMultiprocessor(&ctx->occ_expand_part, expand_kernel<WORDS, kExpandPartition>, ExpandCfg<WORDS>::kThreads, 0)));
-	CU(cudaFuncSetAttribute(expand_fused_kernel<WORDS>, cudaFuncAttributeMaxDynamicSharedMemorySize, FxSmem<WORDS>::kBytes));
 	const size_t cs = count_smem_bytes<WORDS>(ctx->suffix_bytes + ctx->counter_bytes);
 	CU(cudaFuncSetAttribute(count_emit_kernel<WORDS>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)cs));
 	CU(cudaFuncSetAttribute(msd_partition_kernel<WORDS>, cudaFuncAttributeMaxDynamicSharedMemorySize, MsdSmem<WORDS>::kBytes));
@@ -317,7 +299,7 @@ __global__ void msd_setup_kernel(uint64_t* seg1, uint32_t* item_base1, uint32_t*
 
 // bits of the second partition level.  Counted leaves (the bin path) are streamed by one warp and may be any size: a leaf beyond one
 // table round only costs extra rounds, while the 512 / 1024-digit partition kernels are slower per record than the 256-digit one.
-// So: leaves of ~1 K records while that takes <= 8 bits, then ~2 K-record leaves.
+// So: leaves of ~1 K records while that takes <= 8 bits, then (one-word records) leaves of leaf_target records in at most leaf_max_b2 bits.
 // Sorted leaves (seam #1) must fit on chip, and canonical k-mers crowd into the low prefixes (largest leaf ~4.4x the mean): aim at a
 // fifth of the capacity, 8 bits at most.
 template <int WORDS>
@@ -327,12 +309,10 @@ uint32_t choose_b2(const kmcb200_ctx* ctx, uint64_t n, bool counted_leaves)
 	uint32_t b2;
 	if (counted_leaves) {
 		b2 = std::min(bits_for(1024), 10u);
-		// (one-word records only: the leaves of wider records verify every hit against a record in HBM and lose more from a second
-		// table round than the wide scatter costs; scripts/l2_bits_sweep.py, DESIGN 3.1)
-		if (WORDS == 1 && b2 > 8 && !ctx->leaf_hash) b2 = std::max(8u, std::min(bits_for(2048), 10u));
 		// leaf_hash_kernel: a leaf of up to ~2100 records of a 30x bin is ONE table round, and the leaves of a bin spread over 0 .. 2x their mean
-		// (measured over the bin sizes of the target workload with scripts/l2_bits_sweep.py, DESIGN 3.1)
-		if (WORDS == 1 && b2 > 8 && ctx->leaf_hash) b2 = std::max(8u, std::min(bits_for(ctx->leaf_target), ctx->leaf_max_b2));
+		// (measured over the bin sizes of the target workload with scripts/l2_bits_sweep.py, DESIGN 3.1).  One-word records only: the leaves
+		// of wider records verify every hit against a record in HBM and lose more from a second table round than the wide scatter costs.
+		if (WORDS == 1 && b2 > 8) b2 = std::max(8u, std::min(bits_for(ctx->leaf_target), ctx->leaf_max_b2));
 		if (ctx->force_b2) b2 = ctx->force_b2;          // (tests: the wide second level on small bins)
 	} else
 		b2 = std::min(bits_for(std::max<uint64_t>(msd_local_cap<WORDS>() / 5, 64)), 8u);
@@ -444,8 +424,6 @@ int launch_sort(kmcb200_ctx* ctx, Slot& s, void* a, void* b, uint64_t n, uint32_
 		MsdItems items1{};
 		if (hist_ready) {          // items and cells were written by expand_kernel (kExpandAll / kExpandCells)
 			items1.item_lo = s.msd_item_lo1; items1.item_cnt = s.msd_item_cnt1; items1.n_items = &s.zero->status[1];
-		} else if (hist_mode == kHistAligned) {          // the fused expansion counted per aligned tile; its init kernel wrote the one-segment item tables
-			items1.seg_start = s.msd_seg1; items1.item_base = s.msd_item_base1; items1.item_seg = s.msd_item_seg2; items1.n_items = s.msd_item_base1 + 1;
 		} else {
 			msd_setup_kernel<<<1, 1, 0, st>>>(s.msd_seg1, s.msd_item_base1, &s.zero->msd_n_items[0], n, MTILE);
 			items1.seg_start = s.msd_seg1; items1.item_base = s.msd_item_base1; items1.item_seg = s.msd_item_seg2 /* all zero: see below */;
@@ -632,47 +610,9 @@ int stage_expand(kmcb200_ctx* ctx, Slot& s, const uint8_t* d_bin, uint64_t size,
 	const uint32_t np = (n_packs && pack_bytes) ? n_packs : 1;
 	if (!packs_uploaded) if (int rc = upload_packs(ctx, s, size, pack_bytes, n_packs, st)) return rc;
 
-	// ---- KMCB200_EXPAND=fused: one fused pass (expand_fused.cuh) when every pack is a collector flush (<= 64 KiB).  Slower than the
-	// index-based kernels below - a lane that walks its own segment executes the "new record" and the "roll one symbol" paths one after
-	// the other (about twice the warp instructions per k-mer) - so it is an option (no per-super-k-mer index in HBM, two launches fewer),
-	// not the default.
 	bool big_pack = !(n_packs && pack_bytes) && size > (uint64_t)kWalkChunk;
 	if (n_packs && pack_bytes) for (uint32_t i = 0; i < n_packs && !big_pack; ++i) big_pack = pack_bytes[i] > (uint64_t)kWalkChunk;
-	const bool fused = ctx->use_fused && !s.have_extras && em.mode == kExpandAll && !big_pack && n_rec != kExpandUnknownRecs && n_rec < (1ull << 32) && n_rec > 0;
 	s.last_n_packs = np;
-	if (fused) {
-		st = st_expand;
-		const uint32_t nd2 = DISPATCH_WORDS(ctx, choose_nd2, ctx, n_rec, ctx->use_leaf);
-		if (int rc = DISPATCH_WORDS(ctx, ensure_msd, ctx, s, n_rec, np, nd2)) return rc;
-		if (int rc = ensure(ctx, s.pdesc, s.pdesc_cap, (size_t)np + 1, true)) return rc;
-		const uint32_t mtile = ctx->words == 1 ? (uint32_t)msd_tile<1>() : (uint32_t)msd_tile<2>();      // (the same for 2..4 words)
-		static_assert(msd_tile<2>() == msd_tile<3>() && msd_tile<2>() == msd_tile<4>(), "one tile size for all wide records");
-		const uint32_t n_tiles = (uint32_t)((n_rec + mtile - 1) / mtile);
-		uint32_t tile_shift = 0;
-		while ((1u << tile_shift) < mtile) ++tile_shift;
-		InitExtra x;
-		x.cells = reinterpret_cast<uint32_t*>(s.msd_cells); x.cell_words = ((size_t)256 * n_tiles + 1) / 2;
-		x.item_seg = s.msd_item_seg2; x.item_seg_words = (size_t)n_tiles + 2;
-		x.seg1 = s.msd_seg1; x.item_base1 = s.msd_item_base1; x.n = n_rec; x.n_tiles = n_tiles;
-		bin_init_kernel<<<296, 256, 0, st>>>(reinterpret_cast<uint32_t*>(s.zero), (uint32_t)(sizeof(ZeroBlock) / 4), reinterpret_cast<uint32_t*>(zero_lut),
-			(size_t)ctx->lut_entries * 2, reinterpret_cast<uint32_t*>(zero_result), x);
-		FusedArgs f{};
-		f.bin = d_bin; f.size = size; f.pack_start = s.d_pack_start; f.n_packs = np; f.k = k; f.both_strands = ctx->prm.both_strands; f.n_rec = n_rec;
-		f.recs = d_recs; f.cells1 = reinterpret_cast<uint32_t*>(s.msd_cells); f.n_tiles = n_tiles; f.tile_shift = tile_shift;
-		f.top_shift = std::max(2u * k, 8u) - 8u;
-		f.desc = s.pdesc; f.ticket = &s.zero->pack_ticket[0]; f.status = s.zero->status; f.flags = s.zero->msd_flags;
-		if (int rc = next_epoch(ctx, &f.epoch)) return rc;
-		switch (ctx->words) {
-		case 1: expand_fused_kernel<1><<<np, kFxThreads, FxSmem<1>::kBytes, st>>>(f); break;
-		case 2: expand_fused_kernel<2><<<np, kFxThreads, FxSmem<2>::kBytes, st>>>(f); break;
-		case 3: expand_fused_kernel<3><<<np, kFxThreads, FxSmem<3>::kBytes, st>>>(f); break;
-		default: expand_fused_kernel<4><<<np, kFxThreads, FxSmem<4>::kBytes, st>>>(f); break;
-		}
-		ctx->launches += 2;
-		CU(cudaGetLastError());
-		s.hist_mode = kHistAligned;
-		return 0;
-	}
 	const bool cells = em.mode == kExpandAll || em.mode == kExpandCells;          // the expansion writes the level-1 cells
 	s.hist_mode = em.mode == kExpandAll ? kHistTiles : em.mode == kExpandCells ? kHistCells : kHistNone;
 
@@ -703,7 +643,7 @@ int stage_expand(kmcb200_ctx* ctx, Slot& s, const uint8_t* d_bin, uint64_t size,
 	if (em.mode == kExpandCells) s.expand_args = a;
 
 	bin_init_kernel<<<64, 256, 0, st>>>(reinterpret_cast<uint32_t*>(s.zero), (uint32_t)(sizeof(ZeroBlock) / 4), reinterpret_cast<uint32_t*>(zero_lut),
-		(size_t)ctx->lut_entries * 2, reinterpret_cast<uint32_t*>(zero_result), InitExtra());
+		(size_t)ctx->lut_entries * 2, reinterpret_cast<uint32_t*>(zero_result));
 	if (s.have_extras && cells) {          // N4: stage 1 handed over the length bytes: two prefix sums per pack instead of the walk
 		index_from_extras_kernel<<<np, 1024, 0, st>>>(a, s.d_extras, s.d_pack_rec);
 		ctx->launches += 2;
@@ -734,7 +674,7 @@ int stage_count(kmcb200_ctx* ctx, Slot& s, const void* sorted, uint64_t n, uint8
 	uint64_t* d_lut, uint64_t* d_result, cudaStream_t st, bool outputs_zeroed = false, bool guarded = false, const uint64_t* out_base = nullptr)
 {
 	if (!outputs_zeroed) {
-		bin_init_kernel<<<64, 256, 0, st>>>(&s.zero->counters[kMaxPasses], 1u, reinterpret_cast<uint32_t*>(d_lut), (size_t)ctx->lut_entries * 2, reinterpret_cast<uint32_t*>(d_result), InitExtra());
+		bin_init_kernel<<<64, 256, 0, st>>>(&s.zero->counters[kMaxPasses], 1u, reinterpret_cast<uint32_t*>(d_lut), (size_t)ctx->lut_entries * 2, reinterpret_cast<uint32_t*>(d_result));
 		ctx->launches++;
 		CU(cudaGetLastError());
 	}
@@ -790,43 +730,36 @@ int setup_leaf_cta(kmcb200_ctx* ctx)
 // 0.77 ms for a 2^26-k-mer bin, mean leaf 1024, on an H100).
 constexpr uint64_t kLeafCtaMinMean = 1280;
 
-#define DISPATCH_CTA(ctx, fn, ...) ((ctx)->leaf_cta_warps == 8 ? ((ctx)->leaf_cta_slot_bits == 13 ? fn<8, 13>(__VA_ARGS__) : fn<8, 12>(__VA_ARGS__)) \
-                                                             : ((ctx)->leaf_cta_slot_bits == 10 ? fn<4, 10>(__VA_ARGS__) : fn<4, 12>(__VA_ARGS__)))
+#define DISPATCH_CTA(ctx, fn, ...) ((ctx)->leaf_cta_slot_bits == 10 ? fn<4, 10>(__VA_ARGS__) : fn<4, 12>(__VA_ARGS__))
 
 template <int WORDS, int SLOT_BITS>
 int launch_leaves(kmcb200_ctx* ctx, const LeafArgs& la, uint64_t n_rec, cudaStream_t st)
 {
-	if (ctx->leaf_hash && (WORDS == 1 || ctx->leaf_hash_wide)) {
-		const size_t hsmem = sizeof(LhSmem<SLOT_BITS>) * kLwWarps;
-		const uint32_t hgrid = std::min<uint32_t>((la.n_leaves + kLwWarps - 1) / kLwWarps, (uint32_t)(ctx->sm_count * ctx->occ_leaf_hash));
-		// (the usual cutoffs - cutoff_min >= 2, a cutoff_max no count of a leaf reaches - get the instance without the rarely needed transitions)
-		const uint32_t max_count = WORDS == 1 ? kLwHeavy : kLwMaxLeaf;
-		const bool simple = la.cutoff_min >= 2u && la.cutoff_max >= la.cutoff_min && (la.cutoff_max + 1u == 0u || la.cutoff_max + 1u > max_count + 1u);
-		if constexpr (WORDS == 1) {
-			if (ctx->leaf_cta == 1 || (ctx->leaf_cta == 2 && n_rec > kLeafCtaMinMean * la.n_leaves)) DISPATCH_CTA(ctx, launch_leaf_cta, ctx, la, simple, st);
-			else if (simple) leaf_hash_kernel<SLOT_BITS, true><<<hgrid, 32 * kLwWarps, hsmem, st>>>(la);
-			else leaf_hash_kernel<SLOT_BITS, false><<<hgrid, 32 * kLwWarps, hsmem, st>>>(la);
-		} else {
-			if (simple) leaf_hash_wide_kernel<WORDS, SLOT_BITS, true><<<hgrid, 32 * kLwWarps, hsmem, st>>>(la);
-			else leaf_hash_wide_kernel<WORDS, SLOT_BITS, false><<<hgrid, 32 * kLwWarps, hsmem, st>>>(la);
-		}
-		ctx->launches++;
-		CU(cudaGetLastError());
-		return 0;
+	const size_t hsmem = sizeof(LhSmem<SLOT_BITS>) * kLwWarps;
+	const uint32_t hgrid = std::min<uint32_t>((la.n_leaves + kLwWarps - 1) / kLwWarps, (uint32_t)(ctx->sm_count * ctx->occ_leaf_hash));
+	// (the usual cutoffs - cutoff_min >= 2, a cutoff_max no count of a leaf reaches - get the instance without the rarely needed transitions)
+	const uint32_t max_count = WORDS == 1 ? kLwHeavy : kLwMaxLeaf;
+	const bool simple = la.cutoff_min >= 2u && la.cutoff_max >= la.cutoff_min && (la.cutoff_max + 1u == 0u || la.cutoff_max + 1u > max_count + 1u);
+	if constexpr (WORDS == 1) {
+		if (ctx->leaf_cta == 1 || (ctx->leaf_cta == 2 && n_rec > kLeafCtaMinMean * la.n_leaves)) DISPATCH_CTA(ctx, launch_leaf_cta, ctx, la, simple, st);
+		else if (simple) leaf_hash_kernel<SLOT_BITS, true><<<hgrid, 32 * kLwWarps, hsmem, st>>>(la);
+		else leaf_hash_kernel<SLOT_BITS, false><<<hgrid, 32 * kLwWarps, hsmem, st>>>(la);
+	} else {
+		if (simple) leaf_hash_wide_kernel<WORDS, SLOT_BITS, true><<<hgrid, 32 * kLwWarps, hsmem, st>>>(la);
+		else leaf_hash_wide_kernel<WORDS, SLOT_BITS, false><<<hgrid, 32 * kLwWarps, hsmem, st>>>(la);
 	}
-	const size_t smem = sizeof(LwSmem<SLOT_BITS>) * kLwWarps;
-	const uint32_t lgrid = std::min<uint32_t>((la.n_leaves + kLwWarps - 1) / kLwWarps, (uint32_t)(ctx->sm_count * ctx->occ_leaf));
-	leaf_warp_kernel<WORDS, SLOT_BITS><<<lgrid, 32 * kLwWarps, smem, st>>>(la);
 	ctx->launches++;
 	CU(cudaGetLastError());
 	return 0;
 }
 
+// the leaves of one-word records that the leaf kernel only noted (beyond kLwHeavy records: a dominant k-mer)
 template <int WORDS, int SLOT_BITS>
 int launch_heavy_leaves(kmcb200_ctx* ctx, const LeafArgs& la, cudaStream_t st)
 {
+	static_assert(WORDS == 1, "only one-word leaves are noted for the heavy launch");
 	const size_t smem = sizeof(LwSmem<SLOT_BITS>) * kLwWarps;
-	leaf_warp_kernel<WORDS, SLOT_BITS, true><<<(uint32_t)ctx->sm_count, 32 * kLwWarps, smem, st>>>(la);
+	leaf_warp_kernel<SLOT_BITS><<<(uint32_t)ctx->sm_count, 32 * kLwWarps, smem, st>>>(la);
 	ctx->launches++;
 	CU(cudaGetLastError());
 	return 0;
@@ -835,34 +768,27 @@ int launch_heavy_leaves(kmcb200_ctx* ctx, const LeafArgs& la, cudaStream_t st)
 template <int WORDS, int SLOT_BITS>
 int setup_leaves(kmcb200_ctx* ctx)
 {
-	const int smem = (int)(sizeof(LwSmem<SLOT_BITS>) * kLwWarps);
-	CU(cudaFuncSetAttribute(leaf_warp_kernel<WORDS, SLOT_BITS>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
-	CU((cudaFuncSetAttribute(leaf_warp_kernel<WORDS, SLOT_BITS, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem)));
-	CU(cudaFuncSetAttribute(leaf_warp_kernel<WORDS, SLOT_BITS>, cudaFuncAttributePreferredSharedMemoryCarveout, 100));
-	CU(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&ctx->occ_leaf, leaf_warp_kernel<WORDS, SLOT_BITS>, 32 * kLwWarps, smem));
-	if (ctx->occ_leaf < 1) ctx->occ_leaf = 1;
-	{
-		const int hsmem = (int)(sizeof(LhSmem<SLOT_BITS>) * kLwWarps);
-		int occ_t = 1, occ_f = 1;
-		if constexpr (WORDS == 1) {
-			CU((cudaFuncSetAttribute(leaf_hash_kernel<SLOT_BITS, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, hsmem)));
-			CU((cudaFuncSetAttribute(leaf_hash_kernel<SLOT_BITS, true>, cudaFuncAttributePreferredSharedMemoryCarveout, 100)));
-			CU((cudaFuncSetAttribute(leaf_hash_kernel<SLOT_BITS, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, hsmem)));
-			CU((cudaFuncSetAttribute(leaf_hash_kernel<SLOT_BITS, false>, cudaFuncAttributePreferredSharedMemoryCarveout, 100)));
-			CU((cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ_t, leaf_hash_kernel<SLOT_BITS, true>, 32 * kLwWarps, hsmem)));
-			CU((cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ_f, leaf_hash_kernel<SLOT_BITS, false>, 32 * kLwWarps, hsmem)));
-			if (ctx->leaf_cta)
-				if (int rc = DISPATCH_CTA(ctx, setup_leaf_cta, ctx)) return rc;
-		} else {
-			CU((cudaFuncSetAttribute(leaf_hash_wide_kernel<WORDS, SLOT_BITS, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, hsmem)));
-			CU((cudaFuncSetAttribute(leaf_hash_wide_kernel<WORDS, SLOT_BITS, true>, cudaFuncAttributePreferredSharedMemoryCarveout, 100)));
-			CU((cudaFuncSetAttribute(leaf_hash_wide_kernel<WORDS, SLOT_BITS, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, hsmem)));
-			CU((cudaFuncSetAttribute(leaf_hash_wide_kernel<WORDS, SLOT_BITS, false>, cudaFuncAttributePreferredSharedMemoryCarveout, 100)));
-			CU((cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ_t, leaf_hash_wide_kernel<WORDS, SLOT_BITS, true>, 32 * kLwWarps, hsmem)));
-			CU((cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ_f, leaf_hash_wide_kernel<WORDS, SLOT_BITS, false>, 32 * kLwWarps, hsmem)));
-		}
-		ctx->occ_leaf_hash = std::max(1, std::min(occ_t, occ_f));
+	const int hsmem = (int)(sizeof(LhSmem<SLOT_BITS>) * kLwWarps);
+	int occ_t = 1, occ_f = 1;
+	if constexpr (WORDS == 1) {
+		CU((cudaFuncSetAttribute(leaf_warp_kernel<SLOT_BITS>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(sizeof(LwSmem<SLOT_BITS>) * kLwWarps))));
+		CU((cudaFuncSetAttribute(leaf_hash_kernel<SLOT_BITS, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, hsmem)));
+		CU((cudaFuncSetAttribute(leaf_hash_kernel<SLOT_BITS, true>, cudaFuncAttributePreferredSharedMemoryCarveout, 100)));
+		CU((cudaFuncSetAttribute(leaf_hash_kernel<SLOT_BITS, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, hsmem)));
+		CU((cudaFuncSetAttribute(leaf_hash_kernel<SLOT_BITS, false>, cudaFuncAttributePreferredSharedMemoryCarveout, 100)));
+		CU((cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ_t, leaf_hash_kernel<SLOT_BITS, true>, 32 * kLwWarps, hsmem)));
+		CU((cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ_f, leaf_hash_kernel<SLOT_BITS, false>, 32 * kLwWarps, hsmem)));
+		if (ctx->leaf_cta)
+			if (int rc = DISPATCH_CTA(ctx, setup_leaf_cta, ctx)) return rc;
+	} else {
+		CU((cudaFuncSetAttribute(leaf_hash_wide_kernel<WORDS, SLOT_BITS, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, hsmem)));
+		CU((cudaFuncSetAttribute(leaf_hash_wide_kernel<WORDS, SLOT_BITS, true>, cudaFuncAttributePreferredSharedMemoryCarveout, 100)));
+		CU((cudaFuncSetAttribute(leaf_hash_wide_kernel<WORDS, SLOT_BITS, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, hsmem)));
+		CU((cudaFuncSetAttribute(leaf_hash_wide_kernel<WORDS, SLOT_BITS, false>, cudaFuncAttributePreferredSharedMemoryCarveout, 100)));
+		CU((cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ_t, leaf_hash_wide_kernel<WORDS, SLOT_BITS, true>, 32 * kLwWarps, hsmem)));
+		CU((cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ_f, leaf_hash_wide_kernel<WORDS, SLOT_BITS, false>, 32 * kLwWarps, hsmem)));
 	}
+	ctx->occ_leaf_hash = std::max(1, std::min(occ_t, occ_f));
 	return 0;
 }
 
@@ -870,7 +796,7 @@ int setup_leaves(kmcb200_ctx* ctx)
 
 template <int WORDS> int setup_leaves_w(kmcb200_ctx* ctx) { return DISPATCH_SLOTS(ctx, setup_leaves, WORDS, ctx); }
 
-// Partition (two MSD levels), then COUNT the leaves (leaf_hash.cuh / leaf_hash_wide.cuh; leaf_warp.cuh as an option) instead of sorting them; the LSD passes + count_emit_kernel
+// Partition (two MSD levels), then COUNT the leaves (leaf_hash_cta.cuh / leaf_hash.cuh / leaf_hash_wide.cuh, leaf_warp.cuh for a dominant k-mer) instead of sorting them; the LSD passes + count_emit_kernel
 // stand behind as the device-flagged fallback (they return at once unless a leaf could not be counted).
 template <int WORDS>
 int run_sort_count_leaves(kmcb200_ctx* ctx, Slot& s, uint64_t n_rec, uint32_t np_eff, uint8_t* d_out, uint64_t out_capacity, uint64_t* d_lut, uint64_t* d_result, cudaStream_t st,
@@ -894,13 +820,12 @@ int run_sort_count_leaves(kmcb200_ctx* ctx, Slot& s, uint64_t n_rec, uint32_t np
 	const size_t pad = (size_t)((ob + 7) / 8) * 8;
 	if (int rc = ensure(ctx, s.leaf_tmp, s.leaf_tmp_cap, (size_t)n_rec * pad + 64)) return rc;
 	if (!outputs_zeroed) {
-		bin_init_kernel<<<64, 256, 0, st>>>(nullptr, 0u, reinterpret_cast<uint32_t*>(d_lut), (size_t)ctx->lut_entries * 2, reinterpret_cast<uint32_t*>(d_result), InitExtra());
+		bin_init_kernel<<<64, 256, 0, st>>>(nullptr, 0u, reinterpret_cast<uint32_t*>(d_lut), (size_t)ctx->lut_entries * 2, reinterpret_cast<uint32_t*>(d_result));
 		ctx->launches++;
 	}
 	uint32_t* flags = s.zero->msd_flags;
 	LeafArgs la{};
 	la.recs = plan.recs; la.start = plan.start; la.n_leaves = plan.n_leaves; la.low_bits = plan.low_bits;
-	la.round_pct = ctx->leaf_round_pct;
 	la.fill_pct = ctx->leaf_fill_pct; la.ratio0_q8 = ctx->leaf_ratio0_q8;
 	la.leaf_prefix = block_bits ? block_prefix * plan.n_leaves : 0u;          // n_leaves is a power of two
 	la.k = ctx->prm.kmer_len; la.lut_prefix_len = ctx->prm.lut_prefix_len; la.cutoff_min = ctx->prm.cutoff_min; la.cutoff_max = ctx->prm.cutoff_max;
@@ -908,7 +833,7 @@ int run_sort_count_leaves(kmcb200_ctx* ctx, Slot& s, uint64_t n_rec, uint32_t np
 	la.heavy_list = s.zero->heavy_list; la.heavy_count = &s.zero->heavy_count[0]; la.heavy_ticket = &s.zero->heavy_count[1]; la.heavy_cap = kHeavyListCap;
 	la.tmp = s.leaf_tmp; la.leaf_emit = s.leaf_emit; la.group_sum = s.zero->leaf_group_sum; la.lut = d_lut; la.result = d_result; la.ticket = &s.zero->msd_counters[3]; la.flags = flags;
 	if (int rc = DISPATCH_SLOTS(ctx, launch_leaves, WORDS, ctx, la, n_rec, st)) return rc;
-	if (WORDS == 1) {          // the large leaves the main launch only noted (none in a typical bin: the launch returns at once)
+	if constexpr (WORDS == 1) {          // the large leaves the main launch only noted (none in a typical bin: the launch returns at once)
 		if (int rc = DISPATCH_SLOTS(ctx, launch_heavy_leaves, WORDS, ctx, la, st)) return rc;
 	}
 	leaf_scan_kernel<<<(plan.n_leaves + 1023) / 1024, 1024, 0, st>>>(s.leaf_emit, s.zero->leaf_group_sum, plan.n_leaves, s.leaf_off, d_result, out_capacity, ob, flags, out_base);
@@ -948,7 +873,7 @@ int run_bin(kmcb200_ctx* ctx, Slot& s, const uint8_t* d_bin, uint64_t size, uint
 	// a bin of one-word records that takes the MSD path is expanded twice, once to count the level-1 digits, once into the level-1 buckets
 	// (expand.cuh, kExpandCells / kExpandPartition): its records are never written in tile order and read back by a separate partition pass
 	ExpandMode em;
-	if (expand_partition_supported<1>() && ctx->words == 1 && !ctx->use_fused && n_rec < (1ull << 32) && msd_path(ctx, n_rec, 2u * ctx->prm.kmer_len)) em.mode = kExpandCells;
+	if (expand_partition_supported<1>() && ctx->words == 1 && n_rec < (1ull << 32) && msd_path(ctx, n_rec, 2u * ctx->prm.kmer_len)) em.mode = kExpandCells;
 	if (int rc = stage_expand(ctx, s, d_bin, size, n_rec, pack_bytes, n_packs, s.recs_a, st, em, packs_uploaded, d_lut, d_result, st_walk)) return rc;
 	CU(cudaEventRecord(s.ev_expand, st));
 	s.ran_expand = true;
@@ -1279,7 +1204,6 @@ int kmcb200_create(const kmcb200_params* prm, kmcb200_ctx** out_ctx)
 	if (const char* e = getenv("KMCB200_KEY_BLOCKS")) ctx->scatter_blocks = std::string(e) != "filter";
 	if (const char* e = getenv("KMCB200_KEY_BLOCK_RECORDS")) { const long long v = atoll(e); if (v >= 1024) ctx->key_block_records = (uint64_t)v; }
 	if (const char* e = getenv("KMCB200_OVERLAP_WALK")) ctx->overlap_walk = atoi(e) != 0;
-	if (const char* e = getenv("KMCB200_EXPAND")) ctx->use_fused = std::string(e) == "fused";
 	{	// one sort needs two record buffers + the leaves' temporary records (8-byte padded) + ~2 bytes per record of tables: what 60 % of the
 		// free HBM (shared by the context's slots) can hold, below 2^32 records (32-bit record indices inside the kernels)
 		size_t free_b = 0, total_b = 0;
@@ -1292,13 +1216,11 @@ int kmcb200_create(const kmcb200_params* prm, kmcb200_ctx** out_ctx)
 	if (const char* e = getenv("KMCB200_MAX_BLOCK_RECORDS")) { const long long v = atoll(e); if (v >= 1024) ctx->max_block_records = (uint64_t)v; }
 	if (const char* e = getenv("KMCB200_MAX_CHUNK_BYTES")) { const long long v = atoll(e); if (v >= (1 << 17) && v < (1ll << 31)) ctx->max_chunk_bytes = (uint64_t)v; }
 	if (const char* e = getenv("KMCB200_L2_BITS")) { const int v = atoi(e); if (v >= 1 && v <= 10) ctx->force_b2 = (uint32_t)v; }
-	if (const char* e = getenv("KMCB200_LEAF_ROUND_PCT")) { const int v = atoi(e); if (v >= 50 && v <= 1000) ctx->leaf_round_pct = (uint32_t)v; }
-	if (const char* e = getenv("KMCB200_LEAF_KERNEL")) { const std::string v(e); ctx->leaf_hash = v != "warp"; ctx->leaf_cta = v == "cta" ? 1 : v == "warp" || v == "hash" ? 0 : 2; }
+	if (const char* e = getenv("KMCB200_LEAF_KERNEL")) { const std::string v(e); ctx->leaf_cta = v == "cta" ? 1 : v == "hash" ? 0 : 2; }
 	if (const char* e = getenv("KMCB200_LEAF_CTA")) {
 		const std::string v(e);
-		if (v == "4:10" || v == "4:12" || v == "8:12" || v == "8:13") { ctx->leaf_cta_warps = v[0] - '0'; ctx->leaf_cta_slot_bits = atoi(v.c_str() + 2); }
+		if (v == "4:10" || v == "4:12") ctx->leaf_cta_slot_bits = atoi(v.c_str() + 2);
 	}
-	if (const char* e = getenv("KMCB200_LEAF_WIDE")) ctx->leaf_hash_wide = std::string(e) != "warp";
 	if (const char* e = getenv("KMCB200_LEAF_MAX_B2")) { const int v = atoi(e); if (v >= 8 && v <= 10) ctx->leaf_max_b2 = (uint32_t)v; }
 	if (const char* e = getenv("KMCB200_LEAF_TARGET")) { const int v = atoi(e); if (v >= 128 && v <= 8192) ctx->leaf_target = (uint32_t)v; }
 	if (const char* e = getenv("KMCB200_LEAF_FILL_PCT")) { const int v = atoi(e); if (v >= 10 && v <= 85) ctx->leaf_fill_pct = (uint32_t)v; }
@@ -1346,7 +1268,7 @@ void kmcb200_destroy(kmcb200_ctx* ctx)
 	for (auto& s : ctx->slots) {
 		for (void* p : {(void*)s.recs_a, (void*)s.recs_b, (void*)s.recs_x, (void*)s.d_bin, (void*)s.d_pack_start, (void*)s.pack_nsk, (void*)s.pack_nk, (void*)s.pack_tbase,
 				 (void*)s.pack_kbase, (void*)s.pack_done, (void*)s.sk_off, (void*)s.sk_kpre, (void*)s.tile_first, (void*)s.tile_pack, (void*)s.tile_desc, (void*)s.zero, (void*)s.desc,
-				 (void*)s.cdesc, (void*)s.pdesc, (void*)s.d_out, (void*)s.d_lut, (void*)s.d_result, (void*)s.msd_seg1, (void*)s.msd_start2, (void*)s.msd_start3,
+				 (void*)s.cdesc, (void*)s.d_out, (void*)s.d_lut, (void*)s.d_result, (void*)s.msd_seg1, (void*)s.msd_start2, (void*)s.msd_start3,
 				 (void*)s.msd_item_base1, (void*)s.msd_item_base2, (void*)s.msd_item_seg2, (void*)s.msd_item_lo1, (void*)s.msd_item_cnt1,
 				 (void*)s.msd_cells, (void*)s.msd_cell_scan, (void*)s.msd_block_sums, (void*)s.leaf_tmp, (void*)s.leaf_emit, (void*)s.leaf_off, (void*)s.d_hist12, (void*)s.d_out_counter, (void*)s.tot_lut, (void*)s.tot_res, (void*)s.d_extras, (void*)s.d_pack_rec, (void*)s.d_blk_of_prefix, (void*)s.d_region_start})
 			if (p) cudaFree(p);

@@ -14,8 +14,7 @@ from kmc_testlib import fast_bin
 
 K, P, WARM, STEPS = 31, 7, 3, 10
 CONFIGS = [("hash", {"KMCB200_LEAF_KERNEL": "hash"}), ("default", {}), ("cta 4:12", {"KMCB200_LEAF_KERNEL": "cta", "KMCB200_LEAF_CTA": "4:12"}),
-           ("cta 8:12", {"KMCB200_LEAF_KERNEL": "cta", "KMCB200_LEAF_CTA": "8:12"}), ("cta 8:13", {"KMCB200_LEAF_KERNEL": "cta", "KMCB200_LEAF_CTA": "8:13"}),
-           ("cta L2=7", {"KMCB200_LEAF_KERNEL": "cta", "KMCB200_L2_BITS": "7"})]
+           ("cta 4:10", {"KMCB200_LEAF_KERNEL": "cta", "KMCB200_LEAF_CTA": "4:10"}), ("cta L2=7", {"KMCB200_LEAF_KERNEL": "cta", "KMCB200_L2_BITS": "7"})]
 if os.environ.get("SWEEP_CONFIGS"):
     CONFIGS = [c for c in CONFIGS if c[0] in os.environ["SWEEP_CONFIGS"].split(",")]
 dev = torch.device("cuda", 0)

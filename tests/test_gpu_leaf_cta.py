@@ -7,7 +7,7 @@ from kmc_testlib import Bin, Params, fast_bin, pack_superkmers
 
 pytestmark = pytest.mark.gpu
 
-CTA_CONFIGS = ["4:12", "8:12", "8:13", "4:10"]          # KMCB200_LEAF_CTA: warps per CTA : log2(table slots)
+CTA_CONFIGS = ["4:12", "4:10"]                          # KMCB200_LEAF_CTA: warps per CTA : log2(table slots)
 
 
 def _ctx(p: Params):

@@ -56,15 +56,13 @@ def test_leaf_hash_cutoff_instances(oracle, k, both, cmin, cmax, cntmax):
 
 
 @pytest.mark.parametrize("env", [{"KMCB200_LEAF_FILL_PCT": "10"}, {"KMCB200_LEAF_RATIO0": "8"}, {"KMCB200_LEAF_RATIO0": "256", "KMCB200_LEAF_FILL_PCT": "85"},
-                                 {"KMCB200_L2_BITS": "2"}, {"KMCB200_L2_BITS": "2", "KMCB200_LEAF_RATIO0": "8", "KMCB200_LEAF_SLOT_BITS": "8"},
-                                 {"KMCB200_LEAF_KERNEL": "warp"}, {"KMCB200_LEAF_WIDE": "warp"}])
+                                 {"KMCB200_L2_BITS": "2"}, {"KMCB200_L2_BITS": "2", "KMCB200_LEAF_RATIO0": "8", "KMCB200_LEAF_SLOT_BITS": "8"}])
 @pytest.mark.parametrize("coverage", ["30x", "distinct"])
 @pytest.mark.parametrize("k", [31, 55])
 def test_leaf_hash_round_planning(oracle, monkeypatch, env, coverage, k):
     """leaf_hash_kernel plans its table rounds from a running estimate of distinct k-mers per record: rounds planned far too small (many
     predicated rounds over the leaf), far too large (the table fills up: the round is split on the next bit, binary descent), leaves of
-    ~10^4 records in 256-slot tables, duplicate-rich and all-distinct k-mers, one-word and two-word records (leaf_hash_wide_kernel); and the
-    round-1 kernel (leaf_warp_kernel) stays selectable."""
+    ~10^4 records in 256-slot tables, duplicate-rich and all-distinct k-mers, one-word and two-word records (leaf_hash_wide_kernel)."""
     for k_, v in env.items():
         monkeypatch.setenv(k_, v)
     p = Params(k=k, cutoff_min=2 if coverage == "30x" else 1, lut_prefix_len=7)
@@ -496,23 +494,6 @@ def test_lsd_fallback_is_one_cooperative_launch(oracle, monkeypatch, k, p_len):
     ctx.close()
     monkeypatch.setenv("KMCB200_SORT", "lsd")                      # and the plain LSD sort (the same cooperative kernel, always on)
     _check_bin(oracle, fast_bin(9, 31, 250000), Params(k=31, cutoff_min=2, lut_prefix_len=7))
-
-
-@pytest.mark.parametrize("k,both,cmin,p_len,n", [(31, True, 2, 7, 300000), (31, False, 1, 11, 200000), (55, True, 2, 7, 150000), (70, True, 1, 6, 90000), (128, True, 1, 8, 60000),
-                                                 (17, True, 1, 5, 250000), (9, True, 1, 5, 120000), (31, True, 2, 7, 3_000_000)])
-def test_fused_expansion_option(oracle, monkeypatch, k, both, cmin, p_len, n):
-    """KMCB200_EXPAND=fused: walk, look-back and rolling expansion in one kernel per pack (expand_fused.cuh), aligned level-1 cells."""
-    monkeypatch.setenv("KMCB200_EXPAND", "fused")
-    p = Params(k=k, both_strands=both, cutoff_min=cmin, lut_prefix_len=p_len)
-    _check_bin(oracle, fast_bin(900 + k, k, n), p)
-    ctx = _ctx(p)                                   # malformed bins are stopped on the device in this path too
-    import kmc_b200
-    b = fast_bin(901, k, 200000)
-    with pytest.raises(kmc_b200.KmcB200Error) as ei:
-        ctx.process_bin(kmc_b200.SuperKmerBin(data=b.data, n_rec=150000, pack_bytes=b.pack_bytes, kmer_len=k))
-    assert ei.value.code == kmc_b200.ERR_BIN_FORMAT
-    _check_bin(oracle, synth_bin(5, k, 5000, genome_len=20000), p, ctx)
-    ctx.close()
 
 
 @pytest.mark.parametrize("k,p_len,n,n_ctx", [(31, 7, 3_000_000, 2), (31, 7, 1_500_000, 3), (55, 7, 1_200_000, 2), (17, 5, 900_000, 4)])

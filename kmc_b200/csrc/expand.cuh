@@ -67,7 +67,10 @@ struct ExpandArgs {
 	uint64_t* item_lo1;          // [total_tiles] first output record of the tile
 	uint16_t* item_cnt1;         // [total_tiles]
 	uint32_t top_shift;
-	const uint32_t* cell_scan;   // kExpandPartition: exclusive scan of cells1 = output index of (tile, digit) in recs
+	// kExpandPartition (the bin path of one-word records): the level-1 buckets come from digit totals the index kernels count
+	uint32_t* l1_total;          // [256] when set, the walk adds the level-1 digit of every k-mer here
+	uint32_t* l1_cursor;         // [256] next free record of every level-1 bucket (msd_bounds_kernel starts it at l1_start[d])
+	const uint64_t* l1_start;    // [257] level-1 bucket boundaries
 	// oversized bins (kmc_b200.cu, run_oversized_bin): the bin is expanded chunk by chunk, once to count and once per key block
 	uint32_t mode;               // 0: everything (above); 1: only count the top 12 bits into hist12; 2: only k-mers of one key block, appended to recs
 	uint32_t fshift, fprefix, fmask;    // mode 2: keep the k-mers with ((kmer >> fshift) & fmask) == fprefix
@@ -78,11 +81,12 @@ struct ExpandArgs {
 	const uint64_t* region_start;        // [n_blocks] first record of every block's region inside recs
 	uint32_t n_blocks;                   // <= kExpandMaxBlocks
 };
-// kExpandCells + kExpandPartition: the bin path expands a bin of one-word records twice instead of writing the records in tile order and
-// partitioning them by their top digit afterwards.  kExpandCells only counts the level-1 digits of every tile into the cell layout; after
-// the cell scan, kExpandPartition extracts the k-mers again and writes each one to its level-1 bucket (the work of msd_partition_kernel,
-// with the extraction in place of the load).  The tile-ordered copy of the records (8N bytes written, 8N read back) never exists.
-enum : uint32_t { kExpandAll = 0, kExpandCount12 = 1, kExpandFilter = 2, kExpandScatter = 3, kExpandCells = 4, kExpandPartition = 5 };
+// kExpandPartition: the bin path expands a bin of one-word records straight into its level-1 buckets instead of writing the records in
+// tile order and partitioning them by their top digit afterwards.  The pack walk counts the level-1 digit of every k-mer into 256 totals,
+// msd_bounds_kernel turns them into the bucket boundaries, and every tile of the expansion reserves its run inside each bucket with one
+// global atomicAdd (an MSD partition need not be stable, so the order of the runs does not matter).  The tile-ordered copy of the
+// records (8N bytes written, 8N read back) never exists, and the bin is expanded once.
+enum : uint32_t { kExpandAll = 0, kExpandCount12 = 1, kExpandFilter = 2, kExpandScatter = 3, kExpandPartition = 4 };
 // kExpandPartition regroups a tile in shared memory over the staged bytes (8 bytes * 4096 records); wider records would need a larger
 // buffer than static shared memory allows and more registers for the keys it holds
 template <int WORDS> __host__ __device__ constexpr bool expand_partition_supported() { return WORDS == 1; }
@@ -93,6 +97,34 @@ enum : uint32_t { kErrPackWalk = 1, kErrRecCount = 2 };
 constexpr uint32_t kExpandAbortFlag = 2;      // = kMsdFlagAbort (msd_sort.cuh)
 
 __device__ __forceinline__ uint64_t tile_first_base(uint64_t pack_start, uint32_t p, uint32_t tile) { return pack_start * 4 / tile + p; }
+
+// Level-1 digits of the x + 1 k-mers of one super-k-mer whose packed symbols start at `sym` (2 bits per symbol, the first in bits 7-6),
+// added to the 256-entry histogram `hist`.  The digit is the top 8 bits of min(k-mer, reverse complement) of a k-mer of 2k >= 24 bits:
+// min(its first 4 symbols, the complement of its last 4 reversed), or the first 4 alone in -b mode.  Four k-mers at a time: symbols
+// s .. s+7 (bytes s/4 and s/4 + 1) hold the forward digits of k-mers s .. s+3, symbols s+k-4 .. s+k+3 (reversed and complemented once)
+// their reverse ones, so four k-mers cost five byte loads and no chain runs from one group to the next.  The last group may read up to
+// two bytes past the super-k-mer (the next record, or the slack behind the pack); those digits are not counted.
+__device__ __forceinline__ void count_l1_digits(const uint8_t* sym, uint32_t x, uint32_t k, bool both_strands, uint32_t* hist)
+{
+	for (uint32_t s = 0; s <= x; s += 4) {
+		const uint32_t fw = ((uint32_t)sym[s >> 2] << 8) | sym[(s >> 2) + 1];            // symbols s .. s+7, s at bits 15-14
+		uint32_t rw = 0;
+		if (both_strands) {
+			const uint32_t b = s + k - 4, q = b >> 2;
+			const uint32_t v = (((uint32_t)sym[q] << 16) | ((uint32_t)sym[q + 1] << 8) | sym[q + 2]) >> (8u - 2u * (b & 3u));     // symbols b .. b+7 in bits 15..0
+			const uint32_t y = __brev(v) >> 16;                                            // bit order reversed ...
+			rw = ~(((y >> 1) & 0x5555u) | ((y & 0x5555u) << 1));                          // ... symbol order reversed, complemented: b+i at bits 2i+1..2i
+		}
+		const uint32_t n = min(x + 1 - s, 4u);
+#pragma unroll
+		for (uint32_t j = 0; j < 4; ++j) {
+			if (j < n) {
+				const uint32_t f = (fw >> (8u - 2u * j)) & 0xFFu;
+				atomicAdd(&hist[both_strands ? min(f, (rw >> (2u * j)) & 0xFFu) : f], 1u);
+			}
+		}
+	}
+}
 
 // ---------------------------------------------------------------------------------------------------------------------
 // Walking a pack is a serial chain (the length byte of a record says where the next record starts).  For the usual pack
@@ -117,10 +149,13 @@ __global__ void __launch_bounds__(kWalkSegs, 3) walk_packs_parallel_kernel(const
 	extern __shared__ __align__(16) uint8_t wsm[];               // the pack (+ 16 bytes of slack)
 	__shared__ uint32_t s_entry[kWalkSegs], s_exit[kWalkSegs], s_w[16];
 	__shared__ uint32_t s_bad;
+	__shared__ uint32_t s_hist[256];                             // a.l1_total: the pack's level-1 digits
+	static_assert(kWalkSegs == 256, "one histogram entry per thread");
 	const uint32_t p = blockIdx.x, tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
 	const uint64_t pstart = a.pack_start[p];
 	const uint32_t len = (uint32_t)min(a.pack_start[p + 1] - pstart, (uint64_t)kWalkChunk + 1);
 	if (len > (uint32_t)kWalkChunk || len == 0) { if (tid == 0) pack_done[p] = len == 0 ? 1u : 0u; if (len == 0 && tid == 0) { a.pack_nsk[p] = 0; a.pack_nk[p] = 0; } return; }
+	s_hist[tid] = 0;
 	// ---- the pack into shared memory (16-byte loads on the absolute 16-byte grid)
 	{
 		const uintptr_t g0 = reinterpret_cast<uintptr_t>(a.bin + pstart);
@@ -186,7 +221,7 @@ __global__ void __launch_bounds__(kWalkSegs, 3) walk_packs_parallel_kernel(const
 		uint32_t br = ir - nrec, bk = ik - nk, tr = 0, tk = 0;
 #pragma unroll
 		for (int w = 0; w < 8; ++w) { if ((uint32_t)w < warp) { br += s_w[w]; bk += s_w[8 + w]; } tr += s_w[w]; tk += s_w[8 + w]; }
-		// ---- second walk of the own segment: the index
+		// ---- second walk of the own segment: the index (and the level-1 digits of the pack's k-mers)
 		const uint64_t slot = pstart / a.min_rec_bytes;
 		const uint64_t tfb = tile_first_base(pstart, p, a.tile);
 		uint32_t j = br, kk = bk;
@@ -197,11 +232,16 @@ __global__ void __launch_bounds__(kWalkSegs, 3) walk_packs_parallel_kernel(const
 			a.sk_kpre[slot + j] = kk;
 			const uint32_t tb = (kk + a.tile - 1) / a.tile;                     // first tile boundary at or after this super-k-mer's first k-mer
 			if (tb * a.tile < kk + x + 1) a.tile_first[tfb + tb] = j;
+			if (a.l1_total) count_l1_digits(pk + pos + 1, x, a.k, a.both_strands != 0, s_hist);
 			kk += x + 1;
 			pos += 1 + ((x + k3) >> 2);
 			++j;
 		}
 		if (tid == 0) { a.pack_nsk[p] = tr; a.pack_nk[p] = tk; pack_done[p] = 1; }
+		if (a.l1_total) {
+			__syncthreads();
+			if (s_hist[tid]) atomicAdd(&a.l1_total[tid], s_hist[tid]);
+		}
 	}
 }
 
@@ -236,7 +276,9 @@ __global__ void __launch_bounds__(32 * kWalkWarpsPerBlock) walk_packs_kernel(con
 	uint4 cur = walk_load_window(bin_aligned, wbase, limit, lane);
 	uint4 nxt = walk_load_window(bin_aligned, wbase + 512, limit, lane);
 	uint32_t j = 0, nk = 0, next_tile = 0;
-	uint32_t my_off = 0, my_kpre = 0;
+	uint32_t my_off = 0, my_kpre = 0, my_x = 0;
+	// a.l1_total: every lane counts the level-1 digits of the super-k-mers it stores, from global memory (packs this large are rare)
+	auto count = [&]() { if (a.l1_total) count_l1_digits(a.bin + my_off + 1, my_x, a.k, a.both_strands != 0, a.l1_total); };
 	while (pos < end) {
 		uint64_t rel = pos + shift - wbase;
 		if (rel >= 512) {            // a record is at most 1 + (k + 255 + 3) / 4 <= 97 bytes: one window shift is enough
@@ -250,10 +292,11 @@ __global__ void __launch_bounds__(32 * kWalkWarpsPerBlock) walk_packs_kernel(con
 		uint32_t w = comp == 0 ? cur.x : comp == 1 ? cur.y : comp == 2 ? cur.z : cur.w;
 		w = __shfl_sync(0xffffffffu, w, r >> 4);
 		const uint32_t x = (w >> ((r & 3u) * 8u)) & 0xFFu;
-		if (lane == (j & 31u)) { my_off = (uint32_t)pos; my_kpre = nk; }
+		if (lane == (j & 31u)) { my_off = (uint32_t)pos; my_kpre = nk; my_x = x; }
 		if ((j & 31u) == 31u) {      // 32 super-k-mers collected: one coalesced store each
 			a.sk_off[slot + j - 31 + lane] = my_off;
 			a.sk_kpre[slot + j - 31 + lane] = my_kpre;
+			count();
 		}
 		if (nk + x + 1 > next_tile * a.tile) {   // this super-k-mer holds k-mer number next_tile * tile of the pack
 			if (lane == 0) a.tile_first[tfb + next_tile] = j;
@@ -266,6 +309,7 @@ __global__ void __launch_bounds__(32 * kWalkWarpsPerBlock) walk_packs_kernel(con
 	if (lane < (j & 31u)) {          // the unfinished group
 		a.sk_off[slot + (j & ~31u) + lane] = my_off;
 		a.sk_kpre[slot + (j & ~31u) + lane] = my_kpre;
+		count();
 	}
 	if (lane == 0) {
 		if (pos != end) atomicOr(a.status, kErrPackWalk);
@@ -285,6 +329,7 @@ __global__ void __launch_bounds__(1024) index_from_extras_kernel(const ExpandArg
 	__shared__ uint32_t s_b[32], s_k[32];
 	__shared__ uint32_t carry_b, carry_k;
 	__shared__ uint32_t s_bad;
+	__shared__ uint32_t s_hist[256];          // a.l1_total: the pack's level-1 digits
 	const uint32_t p = blockIdx.x, tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
 	const uint64_t pstart = a.pack_start[p];
 	const uint32_t len = (uint32_t)min(a.pack_start[p + 1] - pstart, (uint64_t)0xffffffffu);
@@ -292,6 +337,7 @@ __global__ void __launch_bounds__(1024) index_from_extras_kernel(const ExpandArg
 	const uint32_t nrec = (uint32_t)min(pack_rec_start[p + 1] - r0, (uint64_t)0xffffffffu);
 	const uint64_t slot = pstart / a.min_rec_bytes;
 	const uint64_t tfb = tile_first_base(pstart, p, a.tile);
+	if (tid < 256) s_hist[tid] = 0;
 	if (tid == 0) { carry_b = 0; carry_k = 0; s_bad = 0; }
 	__syncthreads();
 	// (more records than the pack's bytes can hold: the array is wrong; also keeps the index writes inside the pack's own slots)
@@ -318,18 +364,20 @@ __global__ void __launch_bounds__(1024) index_from_extras_kernel(const ExpandArg
 				a.sk_kpre[slot + j] = kk;
 				const uint32_t tb = (kk + a.tile - 1) / a.tile;
 				if (tb * a.tile < kk + x + 1) a.tile_first[tfb + tb] = j;
+				if (a.l1_total) count_l1_digits(a.bin + pstart + off + 1, x, a.k, a.both_strands != 0, s_hist);
 			}
 		}
 		__syncthreads();
 		if (tid == 1023) { carry_b = bb + ib; carry_k = bk + ik; }
 		__syncthreads();
 	}
+	const bool bad = too_many || s_bad || carry_b != len;          // (uniform: the last barrier is behind every write of these)
 	if (tid == 0) {
-		const bool bad = too_many || s_bad || carry_b != len;
 		if (bad) atomicOr(a.status, kErrPackWalk);
 		a.pack_nsk[p] = bad ? 0u : nrec;
 		a.pack_nk[p] = bad ? 0u : carry_k;
 	}
+	if (a.l1_total && !bad && tid < 256 && s_hist[tid]) atomicAdd(&a.l1_total[tid], s_hist[tid]);          // (a malformed pack counts nothing)
 }
 
 // single CTA: exclusive scans over packs
@@ -563,15 +611,13 @@ __global__ void __launch_bounds__(ExpandCfg<WORDS>::kThreads, expand_min_blocks<
 		if (a.flags[1] & kExpandAbortFlag) return;       // (a malformed bin also has no tiles)
 	if (tid < 256) htop[tid] = 0;
 	const uint32_t total_tiles = a.status[1];
+	// (kExpandPartition runs at its register limit: it re-reads the tile count, written by scan_packs_kernel, instead of holding it)
+	auto tiles = [&]() { return MODE == kExpandPartition ? __ldg(a.status + 1) : total_tiles; };
 	Rec<WORDS>* __restrict__ out = reinterpret_cast<Rec<WORDS>*>(a.recs);
 
-	for (uint32_t g = blockIdx.x; g < total_tiles; g += gridDim.x) {
-		// kExpandPartition: output index of this tile's records of digit tid (cell tid * tiles + g), in flight during the tile's set-up
-		uint32_t digit_base = 0;
-		if constexpr (MODE == kExpandPartition)
-			if (tid < 256) digit_base = __ldg(a.cell_scan + g + (size_t)tid * total_tiles);
+	for (uint32_t g = blockIdx.x; g < tiles(); g += gridDim.x) {
 		const uint4 da = __ldg(a.tile_desc + 2 * (size_t)g), db = __ldg(a.tile_desc + 2 * (size_t)g + 1);
-		if (g + gridDim.x < total_tiles) asm volatile("prefetch.global.L2 [%0];" ::"l"(a.tile_desc + 2 * (size_t)(g + gridDim.x)));
+		if (g + gridDim.x < tiles()) asm volatile("prefetch.global.L2 [%0];" ::"l"(a.tile_desc + 2 * (size_t)(g + gridDim.x)));
 		const uint64_t slot0 = da.x;
 		const uint32_t nsk = da.y;
 		const uint32_t j_lo = da.z;
@@ -640,30 +686,14 @@ __global__ void __launch_bounds__(ExpandCfg<WORDS>::kThreads, expand_min_blocks<
 			return extract_kmer<WORDS>(a.bin + off[j] + 1, s, a.k, a.both_strands != 0,
 				[](uintptr_t wa) { return __ldg(reinterpret_cast<const unsigned long long*>(wa)); });
 		};
-		// kExpandCells needs only the top digit of min(kmer, revcomp) = min(its first 4 symbols, the complement of its last 4 reversed):
-		// two 8-bit windows of the staged stream instead of the whole k-mer and its reverse complement (one-word records, k >= 4)
-		auto top_digit_of = [&](uint32_t slot) -> uint32_t {
-			if (WORDS > 1 || !staged || a.top_shift + 8u != 2u * a.k) return rec_top_digit<WORDS>(kmer_of(slot), a.top_shift);
-			const uint32_t rel = hpre[slot >> 5] + __popc(hbits[slot >> 5] & le_mask);
-			const uint32_t B = s_bit[rel] + 2u * slot;
-			const uint32_t* sw = reinterpret_cast<const uint32_t*>(s_bytes);
-			auto byte_at = [&](uint32_t b) { const uint32_t wi = b >> 5; return __funnelshift_l(sw[wi + 1], sw[wi], b & 31u) >> 24; };
-			const uint32_t f = byte_at(B);
-			if (!a.both_strands) return f;
-			uint32_t r = ~byte_at(B + 2u * a.k - 8u) & 0xFFu;
-			r = ((r & 0x03u) << 6) | ((r & 0x0Cu) << 2) | ((r & 0x30u) >> 2) | ((r & 0xC0u) >> 6);
-			return min(f, r);
-		};
-		if constexpr (MODE == kExpandAll || MODE == kExpandCells) {
+		if constexpr (MODE == kExpandAll) {
 #pragma unroll kExpandUnroll
 			for (int i = 0; i < IPT; ++i) {
 				const uint32_t slot = i * kExpandThreads + tid;
 				if (slot < cnt) {
-					if constexpr (MODE == kExpandAll) {
-						const Rec<WORDS> r = kmer_of(slot);
-						out[obase + slot] = r;
-						atomicAdd(&htop[rec_top_digit<WORDS>(r, a.top_shift)], 1u);
-					} else atomicAdd(&htop[top_digit_of(slot)], 1u);          // (counts only: kExpandPartition writes the records)
+					const Rec<WORDS> r = kmer_of(slot);
+					out[obase + slot] = r;
+					atomicAdd(&htop[rec_top_digit<WORDS>(r, a.top_shift)], 1u);
 				}
 			}
 			__syncthreads();
@@ -675,8 +705,8 @@ __global__ void __launch_bounds__(ExpandCfg<WORDS>::kThreads, expand_min_blocks<
 			if (tid == 0) { a.item_lo1[g] = obase; a.item_cnt1[g] = (uint16_t)cnt; }
 		} else if constexpr (MODE == kExpandPartition) {
 			// level-1 partition of the tile straight from the bin (msd_partition_kernel's consumer, with the extraction in place of the load):
-			// rank inside (tile, digit) = return value of one shared-memory atomicAdd, scan of the digit counts, regroup by digit in shared
-			// memory, digit-contiguous runs leave with coalesced stores
+			// rank inside (tile, digit) = return value of one shared-memory atomicAdd, the tile's run inside every bucket = return value of
+			// one global atomicAdd, scan of the digit counts, regroup by digit in shared memory, digit-contiguous runs leave with coalesced stores
 			__shared__ uint32_t s_excl[256], s_goff[256];
 			Rec<WORDS> key[IPT];
 			uint32_t rank[IPT / 2] = {};          // two 16-bit ranks per register (a tile holds at most 4096 records)
@@ -689,10 +719,11 @@ __global__ void __launch_bounds__(ExpandCfg<WORDS>::kThreads, expand_min_blocks<
 				}
 			}
 			__syncthreads();
-			uint32_t c = 0, inc = 0;
+			uint32_t c = 0, inc = 0, base = 0;
 			if (tid < 256) {          // (warps 0..7; every thread zeroes its own digit for the next tile)
 				c = htop[tid];
 				htop[tid] = 0;
+				if (c) base = atomicAdd(&a.l1_cursor[tid], c);          // (issued first: its latency hides behind the scan)
 				inc = c;
 #pragma unroll
 				for (int o = 1; o < 32; o <<= 1) {
@@ -702,14 +733,19 @@ __global__ void __launch_bounds__(ExpandCfg<WORDS>::kThreads, expand_min_blocks<
 				if (lane == 31) warp_max[warp] = inc;
 			}
 			__syncthreads();
+			bool overrun = false;
 			if (tid < 256) {
 				uint32_t ex = inc - c;
 #pragma unroll
 				for (int w = 0; w < 8; ++w) if ((uint32_t)w < warp) ex += warp_max[w];
 				s_excl[tid] = ex;
-				s_goff[tid] = digit_base - ex;          // global index of tile-sorted position q is s_goff[d] + q
+				s_goff[tid] = base - ex;          // global index of tile-sorted position q is s_goff[d] + q
+				// a run beyond its bucket: the walk's totals and this expansion disagree (a bug, never valid input).  The bin then ends as
+				// a reported error, and the tile writes nothing.  (The boundaries of a bin of < 2^32 records fit in 32 bits.)
+				overrun = c && (uint64_t)base + c > (uint32_t)__ldg(a.l1_start + tid + 1);
+				if (overrun) { atomicOr(a.status, kErrRecCount); atomicOr(&a.flags[0], kExpandAbortFlag); atomicOr(&a.flags[1], kExpandAbortFlag); }
 			}
-			__syncthreads();
+			if (__syncthreads_or(overrun)) continue;
 			// every k-mer of the tile is in registers: the staged bytes are free for the regrouping (the next tile stages after a barrier)
 			Rec<WORDS>* buf = reinterpret_cast<Rec<WORDS>*>(s_bytes);
 #pragma unroll

@@ -43,9 +43,9 @@ constexpr uint32_t kHeavyListCap = 2048;           // leaves of more than kLwHea
 
 thread_local std::string g_create_error;
 
-// level-1 cells: none yet / per expand tile (expand.cuh) / per expand tile, and the records are not written yet: the level-1 partition
-// expands the bin a second time (expand_kernel<kExpandPartition>) with the arguments kept in Slot::expand_args
-enum { kHistNone = 0, kHistTiles = 1, kHistCells = 2 };
+// what the expand stage left for level 1: nothing / cells per expand tile (expand.cuh) / the 256 digit totals of the pack walk, and the
+// records are not written yet: the level-1 partition expands the bin (expand_kernel<kExpandPartition>) with the arguments kept in Slot::expand_args
+enum { kHistNone = 0, kHistTiles = 1, kHistTotals = 2 };
 
 struct ZeroBlock {                                // zeroed with one memset at the start of every bin
 	uint64_t hist[kHistRows][256];
@@ -57,6 +57,8 @@ struct ZeroBlock {                                // zeroed with one memset at t
 	uint32_t heavy_count[2];                      // [0] large leaves noted by the leaf kernel, [1] ticket of the second (HEAVY) launch
 	uint32_t heavy_list[kHeavyListCap];           // their leaf ids
 	uint32_t leaf_group_sum[kMaxLeaves / 1024];   // emitted records per group of 1024 leaves
+	uint32_t l1_total[256];                       // kHistTotals: k-mers of every level-1 digit, counted by the pack walk
+	uint32_t l1_cursor[256];                      // kHistTotals: next free record of every level-1 bucket (expand_kernel<kExpandPartition>)
 };
 
 static_assert(sizeof(ZeroBlock) % 4 == 0, "zeroed word by word");
@@ -98,8 +100,8 @@ struct Slot {
 	const char* pass_names[kMaxPasses + 8] = {};
 	uint32_t last_n_packs = 1;
 	uint64_t* cdesc = nullptr; size_t cdesc_cap = 0;        // count look-back descriptors
-	int hist_mode = 0;                                      // what the last expansion left for the sort: kHistNone / kHistTiles / kHistCells
-	ExpandArgs expand_args{};                               // kHistCells: the counting expansion's arguments, for the level-1 partition
+	int hist_mode = 0;                                      // what the last expansion left for the sort: kHistNone / kHistTiles / kHistTotals
+	ExpandArgs expand_args{};                               // kHistTotals: the index's arguments, for the level-1 partition expansion
 	// outputs of the host-buffer path
 	uint8_t* d_out = nullptr; size_t out_cap = 0;
 	uint64_t* d_lut = nullptr;
@@ -273,11 +275,9 @@ int launch_expand(kmcb200_ctx* ctx, const ExpandArgs& a, cudaStream_t st)
 	const uint32_t grid = std::min<uint32_t>(max_tiles, (uint32_t)(ctx->sm_count * (a.mode == kExpandPartition ? std::max(ctx->occ_expand_part, 1) : ctx->occ_expand)));
 	switch (a.mode) {
 	case kExpandAll: expand_kernel<WORDS, kExpandAll><<<grid, ExpandCfg<WORDS>::kThreads, 0, st>>>(a); break;
-	case kExpandCells:
 	case kExpandPartition:
 		if constexpr (expand_partition_supported<WORDS>()) {
-			if (a.mode == kExpandCells) expand_kernel<WORDS, kExpandCells><<<grid, ExpandCfg<WORDS>::kThreads, 0, st>>>(a);
-			else expand_kernel<WORDS, kExpandPartition><<<grid, ExpandCfg<WORDS>::kThreads, 0, st>>>(a);
+			expand_kernel<WORDS, kExpandPartition><<<grid, ExpandCfg<WORDS>::kThreads, 0, st>>>(a);
 			break;
 		} else return fail(ctx, KMCB200_ERR_INVALID, "no level-1 partition expansion for %d-word records", WORDS);
 	case kExpandCount12: expand_kernel<WORDS, kExpandCount12><<<grid, ExpandCfg<WORDS>::kThreads, 0, st>>>(a); break;
@@ -383,8 +383,9 @@ struct LeafPlan {
 bool msd_path(const kmcb200_ctx* ctx, uint64_t n, uint32_t key_bits) { return ctx->use_msd && key_bits >= 24 && n >= (1u << 16); }
 
 // Sorts n records from `a` (with `b` as the second buffer).  *result_in_b tells where the sorted records end up.
-// hist_ready: the expand stage has zeroed the slot's ZeroBlock and written the level-1 cells / items.
-// kHistCells: ... and `a` holds no records yet: the level-1 partition expands them from the bin into `b` (MSD path only).
+// kHistTiles: the expand stage has zeroed the slot's ZeroBlock and written the level-1 cells / items.
+// kHistTotals: it has zeroed the ZeroBlock and counted the level-1 digit totals, and `a` holds no records yet: the level-1 partition
+// expands them from the bin into `b` (MSD path only).
 template <int WORDS>
 int launch_sort(kmcb200_ctx* ctx, Slot& s, void* a, void* b, uint64_t n, uint32_t key_bytes, uint32_t key_bits, int hist_mode, uint32_t n_packs, cudaStream_t st, bool* result_in_b, LeafPlan* plan = nullptr)
 {
@@ -395,12 +396,12 @@ int launch_sort(kmcb200_ctx* ctx, Slot& s, void* a, void* b, uint64_t n, uint32_
 	const uint32_t n_tiles = (uint32_t)n_tiles64;
 	// key_bits: significant bits of a record.  2k for records we expanded ourselves; all key bytes for foreign records (seam #1)
 	const bool msd = msd_path(ctx, n, key_bits);
-	if (hist_mode == kHistCells && !msd) return fail(ctx, KMCB200_ERR_INVALID, "the records of this bin were not expanded");
+	if (hist_mode == kHistTotals && !msd) return fail(ctx, KMCB200_ERR_INVALID, "the records of this bin were not expanded");
 	const uint32_t top_shift = key_bits - 8;
 	if (int rc = ensure(ctx, s.desc, s.desc_cap, (size_t)n_tiles * 256, true)) return rc;
 	if (msd) if (int rc = ensure_msd<WORDS>(ctx, s, n, n_packs, choose_nd2<WORDS>(ctx, n, plan != nullptr))) return rc;      // (sized alike by stage_expand: no reallocation here when its cells are in use)
 
-	const bool hist_ready = hist_mode == kHistTiles || hist_mode == kHistCells;
+	const bool hist_ready = hist_mode == kHistTiles || hist_mode == kHistTotals;
 	if (hist_mode == kHistNone) if (int rc = zero_async(ctx, s.zero, sizeof(ZeroBlock), st)) return rc;
 	int iv = 0;      // timed interval index
 	CU(cudaEventRecord(s.ev_pass[0], st));
@@ -422,9 +423,9 @@ int launch_sort(kmcb200_ctx* ctx, Slot& s, void* a, void* b, uint64_t n, uint32_
 		const int local_smem = msd_local_cap<WORDS>() * 8 * WORDS + (MsdLocalCfg<WORDS>::kThreads / 32) * 1024;
 
 		MsdItems items1{};
-		if (hist_ready) {          // items and cells were written by expand_kernel (kExpandAll / kExpandCells)
+		if (hist_mode == kHistTiles) {          // items and cells were written by expand_kernel<kExpandAll>
 			items1.item_lo = s.msd_item_lo1; items1.item_cnt = s.msd_item_cnt1; items1.n_items = &s.zero->status[1];
-		} else {
+		} else if (hist_mode == kHistNone) {
 			msd_setup_kernel<<<1, 1, 0, st>>>(s.msd_seg1, s.msd_item_base1, &s.zero->msd_n_items[0], n, MTILE);
 			items1.seg_start = s.msd_seg1; items1.item_base = s.msd_item_base1; items1.item_seg = s.msd_item_seg2 /* all zero: see below */;
 			items1.n_items = &s.zero->msd_n_items[0];
@@ -433,29 +434,36 @@ int launch_sort(kmcb200_ctx* ctx, Slot& s, void* a, void* b, uint64_t n, uint32_
 			msd_count_kernel<WORDS><<<(uint32_t)std::min<size_t>(max_items1, (size_t)ctx->sm_count * 4), 512, 0, st>>>(c1);
 			ctx->launches += 2;
 		}
-		if (int rc = launch_cell_scan(ctx, s, items1.n_items, 256, max_items1, never, st)) return rc;
-		s.pass_names[iv] = "msd_scan_L1"; CU(cudaEventRecord(s.ev_pass[++iv], st));
+		if (hist_mode != kHistTotals) {
+			if (int rc = launch_cell_scan(ctx, s, items1.n_items, 256, max_items1, never, st)) return rc;
+			s.pass_names[iv] = "msd_scan_L1"; CU(cudaEventRecord(s.ev_pass[++iv], st));
+		}
 		MsdBoundsArgs b1{};
 		b1.cell_scan = s.msd_cell_scan; b1.items = items1; b1.S = 1; b1.nd = 256; b1.n = n; b1.start = s.msd_start2;
 		b1.cap = b2 == 0 ? cap : 0; b1.flags = flags;
 		b1.tile = b2 > 0 ? MTILE : 0; b1.item_base = s.msd_item_base2; b1.item_seg = s.msd_item_seg2; b1.n_items = &s.zero->msd_n_items[1];
-		MsdPartArgs p1{};
-		p1.in = a; p1.out = b; p1.items = items1; p1.cell_scan = s.msd_cell_scan; p1.shift = top_shift; p1.nd = 256;
-		p1.flags = never;
-		// (the item_seg table of the level-2 items shares its buffer with the all-zero level-1 table: partition first, bounds after)
-		if (hist_mode == kHistCells) {          // the records go from the bin straight into their level-1 buckets in b
+		if (hist_mode == kHistTotals) {          // the records go from the bin straight into their level-1 buckets in b
+			// the buckets (and their cursors) from the walk's digit totals first: the expansion reserves its runs inside them
+			b1.l1_total = s.zero->l1_total; b1.l1_cursor = s.zero->l1_cursor; b1.status = s.zero->status;
+			msd_bounds_kernel<<<1, 1024, 0, st>>>(b1);
+			ctx->launches++;
 			ExpandArgs ea = s.expand_args;
-			ea.mode = kExpandPartition; ea.recs = b; ea.cell_scan = s.msd_cell_scan;
+			ea.mode = kExpandPartition; ea.recs = b; ea.l1_cursor = s.zero->l1_cursor; ea.l1_start = s.msd_start2;
 			if (int rc = launch_expand<WORDS>(ctx, ea, st)) return rc;
 			s.pass_names[iv] = "expand_scatter_L1";
+			CU(cudaEventRecord(s.ev_pass[++iv], st));
 		} else {
+			MsdPartArgs p1{};
+			p1.in = a; p1.out = b; p1.items = items1; p1.cell_scan = s.msd_cell_scan; p1.shift = top_shift; p1.nd = 256;
+			p1.flags = never;
 			msd_partition_kernel<WORDS><<<pgrid1, MsdCfg<WORDS>::kThreads + 32, MsdSmem<WORDS>::kBytes, st>>>(p1);
 			ctx->launches++;
 			s.pass_names[iv] = "msd_partition_L1";
+			CU(cudaEventRecord(s.ev_pass[++iv], st));
+			// (the item_seg table of the level-2 items shares its buffer with the all-zero level-1 table of kHistNone: partition first, bounds after)
+			msd_bounds_kernel<<<1, 1024, 0, st>>>(b1);
+			ctx->launches++;
 		}
-		CU(cudaEventRecord(s.ev_pass[++iv], st));
-		msd_bounds_kernel<<<1, 1024, 0, st>>>(b1);
-		ctx->launches++;
 		if (b2 > 0) {
 			MsdItems items2{};
 			items2.seg_start = s.msd_start2; items2.item_base = s.msd_item_base2; items2.item_seg = s.msd_item_seg2; items2.n_items = &s.zero->msd_n_items[1];
@@ -613,8 +621,9 @@ int stage_expand(kmcb200_ctx* ctx, Slot& s, const uint8_t* d_bin, uint64_t size,
 	bool big_pack = !(n_packs && pack_bytes) && size > (uint64_t)kWalkChunk;
 	if (n_packs && pack_bytes) for (uint32_t i = 0; i < n_packs && !big_pack; ++i) big_pack = pack_bytes[i] > (uint64_t)kWalkChunk;
 	s.last_n_packs = np;
-	const bool cells = em.mode == kExpandAll || em.mode == kExpandCells;          // the expansion writes the level-1 cells
-	s.hist_mode = em.mode == kExpandAll ? kHistTiles : em.mode == kExpandCells ? kHistCells : kHistNone;
+	const uint32_t mode = em.mode;          // (kExpandPartition: the index kernels count the level-1 digits, and no expansion runs here)
+	const bool msd_items = mode == kExpandAll || mode == kExpandPartition;          // level 1 of the sort follows: its buffers are sized here
+	s.hist_mode = mode == kExpandAll ? kHistTiles : mode == kExpandPartition ? kHistTotals : kHistNone;
 
 	if (int rc = ensure(ctx, s.sk_off, s.sk_off_cap, size / min_rec + 2)) return rc;
 	if (int rc = ensure(ctx, s.sk_kpre, s.sk_kpre_cap, size / min_rec + 2)) return rc;
@@ -632,19 +641,20 @@ int stage_expand(kmcb200_ctx* ctx, Slot& s, const uint8_t* d_bin, uint64_t size,
 	a.tile_desc = s.tile_desc;
 	a.status = s.zero->status; a.flags = s.zero->msd_flags;
 	a.recs = d_recs;
-	a.mode = em.mode; a.fshift = em.fshift; a.fprefix = em.fprefix; a.fmask = em.fmask; a.hist12 = em.hist12; a.out_counter = em.out_counter;
+	a.mode = mode; a.fshift = em.fshift; a.fprefix = em.fprefix; a.fmask = em.fmask; a.hist12 = em.hist12; a.out_counter = em.out_counter;
 	a.blk_of_prefix = em.blk_of_prefix; a.region_start = em.region_start; a.n_blocks = em.n_blocks;
-	if (cells) {
+	if (msd_items)
 		if (int rc = DISPATCH_WORDS(ctx, ensure_msd, ctx, s, n_rec, np, DISPATCH_WORDS(ctx, choose_nd2, ctx, n_rec, ctx->use_leaf))) return rc;
-		a.cells1 = s.msd_cells; a.item_lo1 = s.msd_item_lo1; a.item_cnt1 = s.msd_item_cnt1;
-	} else { a.cells1 = nullptr; a.item_lo1 = nullptr; a.item_cnt1 = nullptr; }
+	if (mode == kExpandAll) { a.cells1 = s.msd_cells; a.item_lo1 = s.msd_item_lo1; a.item_cnt1 = s.msd_item_cnt1; }
+	else { a.cells1 = nullptr; a.item_lo1 = nullptr; a.item_cnt1 = nullptr; }
 	a.top_shift = std::max(2u * k, 8u) - 8u;
-	a.cell_scan = nullptr;
-	if (em.mode == kExpandCells) s.expand_args = a;
+	a.l1_total = mode == kExpandPartition ? s.zero->l1_total : nullptr;
+	a.l1_cursor = nullptr; a.l1_start = nullptr;
+	if (mode == kExpandPartition) s.expand_args = a;
 
 	bin_init_kernel<<<64, 256, 0, st>>>(reinterpret_cast<uint32_t*>(s.zero), (uint32_t)(sizeof(ZeroBlock) / 4), reinterpret_cast<uint32_t*>(zero_lut),
 		(size_t)ctx->lut_entries * 2, reinterpret_cast<uint32_t*>(zero_result));
-	if (s.have_extras && cells) {          // N4: stage 1 handed over the length bytes: two prefix sums per pack instead of the walk
+	if (s.have_extras && msd_items) {          // N4: stage 1 handed over the length bytes: two prefix sums per pack instead of the walk
 		index_from_extras_kernel<<<np, 1024, 0, st>>>(a, s.d_extras, s.d_pack_rec);
 		ctx->launches += 2;
 		big_pack = false;
@@ -665,6 +675,7 @@ int stage_expand(kmcb200_ctx* ctx, Slot& s, const uint8_t* d_bin, uint64_t size,
 		CU(cudaEventRecord(s.ev_walk, st));
 		CU(cudaStreamWaitEvent(st_expand, s.ev_walk, 0));
 	}
+	if (mode == kExpandPartition) return 0;          // the bin is expanded by level 1 of the sort, once its buckets are known
 	return DISPATCH_WORDS(ctx, launch_expand, ctx, a, st_expand);
 }
 
@@ -870,10 +881,10 @@ int run_bin(kmcb200_ctx* ctx, Slot& s, const uint8_t* d_bin, uint64_t size, uint
 	}
 	if (int rc = ensure(ctx, s.recs_a, s.recs_a_cap, n_rec * rec_bytes)) return rc;
 	if (int rc = ensure(ctx, s.recs_b, s.recs_b_cap, n_rec * rec_bytes)) return rc;
-	// a bin of one-word records that takes the MSD path is expanded twice, once to count the level-1 digits, once into the level-1 buckets
-	// (expand.cuh, kExpandCells / kExpandPartition): its records are never written in tile order and read back by a separate partition pass
+	// a bin of one-word records that takes the MSD path is expanded once, straight into its level-1 buckets, whose sizes the pack walk
+	// counts (expand.cuh, kExpandPartition): its records are never written in tile order and read back by a separate partition pass
 	ExpandMode em;
-	if (expand_partition_supported<1>() && ctx->words == 1 && n_rec < (1ull << 32) && msd_path(ctx, n_rec, 2u * ctx->prm.kmer_len)) em.mode = kExpandCells;
+	if (expand_partition_supported<1>() && ctx->words == 1 && n_rec < (1ull << 32) && msd_path(ctx, n_rec, 2u * ctx->prm.kmer_len)) em.mode = kExpandPartition;
 	if (int rc = stage_expand(ctx, s, d_bin, size, n_rec, pack_bytes, n_packs, s.recs_a, st, em, packs_uploaded, d_lut, d_result, st_walk)) return rc;
 	CU(cudaEventRecord(s.ev_expand, st));
 	s.ran_expand = true;

@@ -246,7 +246,17 @@ __global__ void __launch_bounds__(32 * kLwWarps, kLwMinBlocks) leaf_warp_kernel(
 		uint32_t n_eq = 0, m_rest = m;
 		const unsigned long long* __restrict__ g = reinterpret_cast<const unsigned long long*>(recs) + lo;
 		if (m > kLwHeavy && m <= kLwMaxHeavyLeaf) {
-			cand = __ldg(g);          // (the first record: a k-mer that holds most of the leaf is very likely to be it; if not, nothing is lost but this scan)
+			// the candidate: the most frequent of 32 evenly spaced records (a k-mer that holds more than a quarter of the leaf is very likely to
+			// be it, whatever the order of the leaf's records - level 1 reserves its runs in no fixed order; if not, nothing is lost but this scan)
+			{
+				const uint64_t smp = __ldg(g + (uint64_t)lane * m / 32);
+				uint32_t votes = 0;
+				for (int i = 0; i < 32; ++i) votes += __shfl_sync(FULL, smp, i) == smp;
+				uint32_t best = (votes << 5) | (31u - lane);          // (ties: the lowest lane)
+#pragma unroll
+				for (int o = 16; o > 0; o >>= 1) best = max(best, __shfl_xor_sync(FULL, best, o));
+				cand = __shfl_sync(FULL, smp, 31u - (best & 31u));
+			}
 			for (uint32_t j0 = 0; j0 < m; j0 += 128) {
 				uint64_t v[4];
 #pragma unroll

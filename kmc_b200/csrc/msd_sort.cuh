@@ -18,6 +18,7 @@
 // returns at once and the 8-bit LSD passes of radix_sort.cuh (always enqueued behind, normally returning at once) sort the bin.
 #pragma once
 #include "common.cuh"
+#include "expand.cuh"
 #include "radix_sort.cuh"
 
 namespace kmcb {
@@ -459,6 +460,11 @@ struct MsdBoundsArgs {
 	uint32_t* item_base;         // [M + 1]
 	uint32_t* item_seg;
 	uint32_t* n_items;
+	// level 1 of the bin path (expand.cuh, kExpandPartition; msd_bounds_kernel only): the boundaries are the exclusive scan of these
+	// 256 digit totals instead of scanned cells, and every bucket's cursor starts at its boundary
+	const uint32_t* l1_total;    // [256] or nullptr
+	uint32_t* l1_cursor;         // [256]
+	uint32_t* status;            // expand status: kErrRecCount when the totals do not add up to n
 };
 
 // boundaries + oversize check only (any number of CTAs): used when no item table is needed
@@ -488,6 +494,27 @@ __global__ void __launch_bounds__(1024) msd_bounds_kernel(const MsdBoundsArgs a)
 	if (*a.flags & kMsdFlagStop) return;
 	const uint32_t M = a.S * a.nd;
 	// pass 1: boundaries.  Buckets of an empty segment (no items, no cells) collapse onto the segment start.
+	if (a.l1_total) {          // (M = 256 digits of one segment, n < 2^32)
+		const uint32_t c = tid < M ? a.l1_total[tid] : 0u;
+		uint32_t inc = c;
+#pragma unroll
+		for (int o = 1; o < 32; o <<= 1) {
+			const uint32_t t = __shfl_up_sync(0xffffffffu, inc, o);
+			if (lane >= (uint32_t)o) inc += t;
+		}
+		if (lane == 31) s_i[warp] = inc;
+		__syncthreads();
+		uint32_t ex = inc - c;
+		for (uint32_t w = 0; w < warp; ++w) ex += s_i[w];
+		if (tid < M) { a.start[tid] = ex; a.l1_cursor[tid] = ex; }
+		if (tid == M) a.start[M] = a.n;
+		if (tid == M - 1) carry_i = ex + c;
+		__syncthreads();
+		if (carry_i != a.n) {          // the walk counted other k-mers than the bin holds (a bug): a bin error, nothing runs behind
+			if (tid == 0) { atomicOr(a.status, kErrRecCount); atomicOr(&a.flags[0], kMsdFlagAbort); atomicOr(&a.flags[1], kMsdFlagAbort); }
+			return;
+		}
+	} else
 	for (uint32_t m = tid; m <= M; m += 1024) {
 		uint64_t v = a.n;
 		if (m < M) {

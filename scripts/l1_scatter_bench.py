@@ -1,12 +1,12 @@
 """Level 1 of a k=31 bin, two ways, on resident bins of bench.py's workload (same generator and seed family), in the library named by
 KMCB200_LIB (default: the package's):
-  new: index + counting expansion (`expand` interval of kmcb200_dev_process_bin) and the expansion that writes every k-mer into its
-       level-1 bucket (`expand_scatter_L1`), the bin path;
+  new: index, whose pack walk counts the level-1 digit totals (`expand` interval of kmcb200_dev_process_bin), and the bucket bounds +
+       the one expansion that writes every k-mer into its level-1 bucket (`expand_scatter_L1`), the bin path;
   old: index + expand_kernel<kExpandAll> (`expand` of kmcb200_dev_expand) and msd_partition_kernel (`msd_partition_L1` of
        kmcb200_dev_sort with hist_ready), the sequence kmcb200_dev_expand's callers still get.
 Every interval is the median of REPS CUDA-event intervals.  The payload, the LUT and the 8 result words of the two paths are compared
 (the old path counts with kmcb200_dev_count).  Algorithmic bytes: S = bin bytes, N = k-mers, 8-byte records:
-  index + count: S;  scatter: S + 8N;  old expand: S + 8N;  old partition: 16N.
+  index + digit totals: S;  scatter: S + 8N;  old expand: S + 8N;  old partition: 16N.
 Usage (GPU): python scripts/l1_scatter_bench.py [k-mers per bin, in Mi or as 2^x ...]"""
 import os
 import subprocess
@@ -89,7 +89,7 @@ def run_size(n_rec, seed):
     same = (r_new == r_old and torch.equal(luts[0], luts[1]) and torch.equal(outs[0][:nb], outs[1][:nb]))
     ctx.close()
     S, N = b.size, n_rec
-    rows = [("new index + count", med(new_idx), S), ("new expand_scatter_L1", med(new_sc), S + 8 * N),
+    rows = [("new index + totals", med(new_idx), S), ("new expand_scatter_L1", med(new_sc), S + 8 * N),
             ("old index + expand", med(old_exp), S + 8 * N), ("old msd_partition_L1", med(old_part), 16 * N)]
     print("n = %d k-mers (%.3g), S = %d bin bytes, %d launches per bin, lsd_fallback %d, results identical: %s, words %s"
           % (N, N, S, launches, r_new[7], same, r_new), flush=True)

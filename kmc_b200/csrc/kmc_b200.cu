@@ -138,20 +138,15 @@ struct kmcb200_ctx {
 	bool use_msd = true;                                    // KMCB200_SORT=lsd forces the plain 8-bit LSD passes
 	bool scatter_blocks = true;                             // KMCB200_KEY_BLOCKS=filter: key blocks always re-expand the bin with a filter (what happens anyway when the records do not fit in HBM once)
 	uint64_t key_block_records = 1ull << 28;                // KMCB200_KEY_BLOCK_RECORDS: preferred size of a key block when the bin is scattered once (leaves of ~1-2 K records)
-	bool overlap_walk = true;                               // KMCB200_OVERLAP_WALK=0: the index kernels of a submitted bin on the compute stream instead of its copy stream
-	bool use_leaf = true;                                   // KMCB200_LEAF=sort sorts the leaves + count_emit instead of counting them
 	int occ_leaf_hash = 1;
 	int leaf_cta = 2;                                       // one-word records by leaf_hash_cta_kernel (one table per CTA): 2 = in bins of mean leaves > kLeafCtaMinMean,
 	                                                        // 1 = always (KMCB200_LEAF_KERNEL=cta), 0 = never (KMCB200_LEAF_KERNEL=hash: leaf_hash_kernel)
 	int leaf_cta_slot_bits = 12;                            // KMCB200_LEAF_CTA = 4:B, the 2^B slots of leaf_hash_cta_kernel's table (4 warps per CTA)
 	int occ_leaf_cta = 1;
-	uint32_t leaf_max_b2 = 8;                               // KMCB200_LEAF_MAX_B2 (8: on the H100 the 512 / 1024-digit level 2 costs more than it saves, DESIGN 3.1)
-	uint32_t leaf_target = 1024;                            // KMCB200_LEAF_TARGET: mean leaf size the second partition level of a large bin aims at (leaf_hash_kernel)
 	uint32_t leaf_fill_pct = 62;                            // KMCB200_LEAF_FILL_PCT: leaf_hash_kernel plans a table round for this load
 	uint32_t leaf_ratio0_q8 = 90;                           // KMCB200_LEAF_RATIO0: first guess of distinct k-mers per record, x 256 (30x coverage, 1 % errors: ~0.3)
 	uint64_t max_block_records = 1ull << 28;                // a bin with more k-mers is counted key block by key block: from the free HBM at create (KMCB200_MAX_BLOCK_RECORDS overrides)
 	uint64_t max_chunk_bytes = 1ull << 30;                  // KMCB200_MAX_CHUNK_BYTES: ... and expanded chunk by chunk
-	int leaf_slot_bits = 10;                                // KMCB200_LEAF_SLOT_BITS = 8 | 9 | 10: slots of a warp's leaf table
 	uint32_t epoch = 1;
 	uint64_t launches = 0;
 	// All kernels of a context run on ONE stream: the persistent radix passes size their grids to fill the GPU and two of
@@ -299,7 +294,9 @@ __global__ void msd_setup_kernel(uint64_t* seg1, uint32_t* item_base1, uint32_t*
 
 // bits of the second partition level.  Counted leaves (the bin path) are streamed by one warp and may be any size: a leaf beyond one
 // table round only costs extra rounds, while the 512 / 1024-digit partition kernels are slower per record than the 256-digit one.
-// So: leaves of ~1 K records while that takes <= 8 bits, then (one-word records) leaves of leaf_target records in at most leaf_max_b2 bits.
+// So: leaves of ~1 K records, in at most 8 bits for one-word records (DESIGN 3.1: on the H100 the wider level 2 costs more than it saves
+// at every bin size of the target workload) and at most 10 bits for wider ones (their leaves verify every hit against a record in HBM and
+// lose more from a second table round than the wide scatter costs).
 // Sorted leaves (seam #1) must fit on chip, and canonical k-mers crowd into the low prefixes (largest leaf ~4.4x the mean): aim at a
 // fifth of the capacity, 8 bits at most.
 template <int WORDS>
@@ -308,11 +305,7 @@ uint32_t choose_b2(const kmcb200_ctx* ctx, uint64_t n, bool counted_leaves)
 	auto bits_for = [&](uint64_t target) { uint32_t lg = 0; while ((1ull << lg) < (n + target - 1) / target) ++lg; return lg > 8 ? lg - 8 : 0u; };
 	uint32_t b2;
 	if (counted_leaves) {
-		b2 = std::min(bits_for(1024), 10u);
-		// leaf_hash_kernel: a leaf of up to ~2100 records of a 30x bin is ONE table round, and the leaves of a bin spread over 0 .. 2x their mean
-		// (measured over the bin sizes of the target workload with scripts/l2_bits_sweep.py, DESIGN 3.1).  One-word records only: the leaves
-		// of wider records verify every hit against a record in HBM and lose more from a second table round than the wide scatter costs.
-		if (WORDS == 1 && b2 > 8) b2 = std::max(8u, std::min(bits_for(ctx->leaf_target), ctx->leaf_max_b2));
+		b2 = std::min(bits_for(1024), WORDS == 1 ? 8u : 10u);
 		if (ctx->force_b2) b2 = ctx->force_b2;          // (tests: the wide second level on small bins)
 	} else
 		b2 = std::min(bits_for(std::max<uint64_t>(msd_local_cap<WORDS>() / 5, 64)), 8u);
@@ -644,7 +637,7 @@ int stage_expand(kmcb200_ctx* ctx, Slot& s, const uint8_t* d_bin, uint64_t size,
 	a.mode = mode; a.fshift = em.fshift; a.fprefix = em.fprefix; a.fmask = em.fmask; a.hist12 = em.hist12; a.out_counter = em.out_counter;
 	a.blk_of_prefix = em.blk_of_prefix; a.region_start = em.region_start; a.n_blocks = em.n_blocks;
 	if (msd_items)
-		if (int rc = DISPATCH_WORDS(ctx, ensure_msd, ctx, s, n_rec, np, DISPATCH_WORDS(ctx, choose_nd2, ctx, n_rec, ctx->use_leaf))) return rc;
+		if (int rc = DISPATCH_WORDS(ctx, ensure_msd, ctx, s, n_rec, np, DISPATCH_WORDS(ctx, choose_nd2, ctx, n_rec, true))) return rc;
 	if (mode == kExpandAll) { a.cells1 = s.msd_cells; a.item_lo1 = s.msd_item_lo1; a.item_cnt1 = s.msd_item_cnt1; }
 	else { a.cells1 = nullptr; a.item_lo1 = nullptr; a.item_cnt1 = nullptr; }
 	a.top_shift = std::max(2u * k, 8u) - 8u;
@@ -741,23 +734,25 @@ int setup_leaf_cta(kmcb200_ctx* ctx)
 // 0.77 ms for a 2^26-k-mer bin, mean leaf 1024, on an H100).
 constexpr uint64_t kLeafCtaMinMean = 1280;
 
+constexpr int kLeafSlotBits = 10;          // a warp's leaf table (leaf_hash_kernel, leaf_hash_wide_kernel, leaf_warp_kernel): 2^10 slots
+
 #define DISPATCH_CTA(ctx, fn, ...) ((ctx)->leaf_cta_slot_bits == 10 ? fn<4, 10>(__VA_ARGS__) : fn<4, 12>(__VA_ARGS__))
 
-template <int WORDS, int SLOT_BITS>
+template <int WORDS>
 int launch_leaves(kmcb200_ctx* ctx, const LeafArgs& la, uint64_t n_rec, cudaStream_t st)
 {
-	const size_t hsmem = sizeof(LhSmem<SLOT_BITS>) * kLwWarps;
+	const size_t hsmem = sizeof(LhSmem<kLeafSlotBits>) * kLwWarps;
 	const uint32_t hgrid = std::min<uint32_t>((la.n_leaves + kLwWarps - 1) / kLwWarps, (uint32_t)(ctx->sm_count * ctx->occ_leaf_hash));
 	// (the usual cutoffs - cutoff_min >= 2, a cutoff_max no count of a leaf reaches - get the instance without the rarely needed transitions)
 	const uint32_t max_count = WORDS == 1 ? kLwHeavy : kLwMaxLeaf;
 	const bool simple = la.cutoff_min >= 2u && la.cutoff_max >= la.cutoff_min && (la.cutoff_max + 1u == 0u || la.cutoff_max + 1u > max_count + 1u);
 	if constexpr (WORDS == 1) {
 		if (ctx->leaf_cta == 1 || (ctx->leaf_cta == 2 && n_rec > kLeafCtaMinMean * la.n_leaves)) DISPATCH_CTA(ctx, launch_leaf_cta, ctx, la, simple, st);
-		else if (simple) leaf_hash_kernel<SLOT_BITS, true><<<hgrid, 32 * kLwWarps, hsmem, st>>>(la);
-		else leaf_hash_kernel<SLOT_BITS, false><<<hgrid, 32 * kLwWarps, hsmem, st>>>(la);
+		else if (simple) leaf_hash_kernel<kLeafSlotBits, true><<<hgrid, 32 * kLwWarps, hsmem, st>>>(la);
+		else leaf_hash_kernel<kLeafSlotBits, false><<<hgrid, 32 * kLwWarps, hsmem, st>>>(la);
 	} else {
-		if (simple) leaf_hash_wide_kernel<WORDS, SLOT_BITS, true><<<hgrid, 32 * kLwWarps, hsmem, st>>>(la);
-		else leaf_hash_wide_kernel<WORDS, SLOT_BITS, false><<<hgrid, 32 * kLwWarps, hsmem, st>>>(la);
+		if (simple) leaf_hash_wide_kernel<WORDS, kLeafSlotBits, true><<<hgrid, 32 * kLwWarps, hsmem, st>>>(la);
+		else leaf_hash_wide_kernel<WORDS, kLeafSlotBits, false><<<hgrid, 32 * kLwWarps, hsmem, st>>>(la);
 	}
 	ctx->launches++;
 	CU(cudaGetLastError());
@@ -765,47 +760,41 @@ int launch_leaves(kmcb200_ctx* ctx, const LeafArgs& la, uint64_t n_rec, cudaStre
 }
 
 // the leaves of one-word records that the leaf kernel only noted (beyond kLwHeavy records: a dominant k-mer)
-template <int WORDS, int SLOT_BITS>
 int launch_heavy_leaves(kmcb200_ctx* ctx, const LeafArgs& la, cudaStream_t st)
 {
-	static_assert(WORDS == 1, "only one-word leaves are noted for the heavy launch");
-	const size_t smem = sizeof(LwSmem<SLOT_BITS>) * kLwWarps;
-	leaf_warp_kernel<SLOT_BITS><<<(uint32_t)ctx->sm_count, 32 * kLwWarps, smem, st>>>(la);
+	const size_t smem = sizeof(LwSmem<kLeafSlotBits>) * kLwWarps;
+	leaf_warp_kernel<kLeafSlotBits><<<(uint32_t)ctx->sm_count, 32 * kLwWarps, smem, st>>>(la);
 	ctx->launches++;
 	CU(cudaGetLastError());
 	return 0;
 }
 
-template <int WORDS, int SLOT_BITS>
+template <int WORDS>
 int setup_leaves(kmcb200_ctx* ctx)
 {
-	const int hsmem = (int)(sizeof(LhSmem<SLOT_BITS>) * kLwWarps);
+	const int hsmem = (int)(sizeof(LhSmem<kLeafSlotBits>) * kLwWarps);
 	int occ_t = 1, occ_f = 1;
 	if constexpr (WORDS == 1) {
-		CU((cudaFuncSetAttribute(leaf_warp_kernel<SLOT_BITS>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(sizeof(LwSmem<SLOT_BITS>) * kLwWarps))));
-		CU((cudaFuncSetAttribute(leaf_hash_kernel<SLOT_BITS, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, hsmem)));
-		CU((cudaFuncSetAttribute(leaf_hash_kernel<SLOT_BITS, true>, cudaFuncAttributePreferredSharedMemoryCarveout, 100)));
-		CU((cudaFuncSetAttribute(leaf_hash_kernel<SLOT_BITS, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, hsmem)));
-		CU((cudaFuncSetAttribute(leaf_hash_kernel<SLOT_BITS, false>, cudaFuncAttributePreferredSharedMemoryCarveout, 100)));
-		CU((cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ_t, leaf_hash_kernel<SLOT_BITS, true>, 32 * kLwWarps, hsmem)));
-		CU((cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ_f, leaf_hash_kernel<SLOT_BITS, false>, 32 * kLwWarps, hsmem)));
+		CU((cudaFuncSetAttribute(leaf_warp_kernel<kLeafSlotBits>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(sizeof(LwSmem<kLeafSlotBits>) * kLwWarps))));
+		CU((cudaFuncSetAttribute(leaf_hash_kernel<kLeafSlotBits, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, hsmem)));
+		CU((cudaFuncSetAttribute(leaf_hash_kernel<kLeafSlotBits, true>, cudaFuncAttributePreferredSharedMemoryCarveout, 100)));
+		CU((cudaFuncSetAttribute(leaf_hash_kernel<kLeafSlotBits, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, hsmem)));
+		CU((cudaFuncSetAttribute(leaf_hash_kernel<kLeafSlotBits, false>, cudaFuncAttributePreferredSharedMemoryCarveout, 100)));
+		CU((cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ_t, leaf_hash_kernel<kLeafSlotBits, true>, 32 * kLwWarps, hsmem)));
+		CU((cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ_f, leaf_hash_kernel<kLeafSlotBits, false>, 32 * kLwWarps, hsmem)));
 		if (ctx->leaf_cta)
 			if (int rc = DISPATCH_CTA(ctx, setup_leaf_cta, ctx)) return rc;
 	} else {
-		CU((cudaFuncSetAttribute(leaf_hash_wide_kernel<WORDS, SLOT_BITS, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, hsmem)));
-		CU((cudaFuncSetAttribute(leaf_hash_wide_kernel<WORDS, SLOT_BITS, true>, cudaFuncAttributePreferredSharedMemoryCarveout, 100)));
-		CU((cudaFuncSetAttribute(leaf_hash_wide_kernel<WORDS, SLOT_BITS, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, hsmem)));
-		CU((cudaFuncSetAttribute(leaf_hash_wide_kernel<WORDS, SLOT_BITS, false>, cudaFuncAttributePreferredSharedMemoryCarveout, 100)));
-		CU((cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ_t, leaf_hash_wide_kernel<WORDS, SLOT_BITS, true>, 32 * kLwWarps, hsmem)));
-		CU((cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ_f, leaf_hash_wide_kernel<WORDS, SLOT_BITS, false>, 32 * kLwWarps, hsmem)));
+		CU((cudaFuncSetAttribute(leaf_hash_wide_kernel<WORDS, kLeafSlotBits, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, hsmem)));
+		CU((cudaFuncSetAttribute(leaf_hash_wide_kernel<WORDS, kLeafSlotBits, true>, cudaFuncAttributePreferredSharedMemoryCarveout, 100)));
+		CU((cudaFuncSetAttribute(leaf_hash_wide_kernel<WORDS, kLeafSlotBits, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, hsmem)));
+		CU((cudaFuncSetAttribute(leaf_hash_wide_kernel<WORDS, kLeafSlotBits, false>, cudaFuncAttributePreferredSharedMemoryCarveout, 100)));
+		CU((cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ_t, leaf_hash_wide_kernel<WORDS, kLeafSlotBits, true>, 32 * kLwWarps, hsmem)));
+		CU((cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ_f, leaf_hash_wide_kernel<WORDS, kLeafSlotBits, false>, 32 * kLwWarps, hsmem)));
 	}
 	ctx->occ_leaf_hash = std::max(1, std::min(occ_t, occ_f));
 	return 0;
 }
-
-#define DISPATCH_SLOTS(ctx, fn, W, ...) ((ctx)->leaf_slot_bits == 8 ? fn<W, 8>(__VA_ARGS__) : (ctx)->leaf_slot_bits == 10 ? fn<W, 10>(__VA_ARGS__) : fn<W, 9>(__VA_ARGS__))
-
-template <int WORDS> int setup_leaves_w(kmcb200_ctx* ctx) { return DISPATCH_SLOTS(ctx, setup_leaves, WORDS, ctx); }
 
 // Partition (two MSD levels), then COUNT the leaves (leaf_hash_cta.cuh / leaf_hash.cuh / leaf_hash_wide.cuh, leaf_warp.cuh for a dominant k-mer) instead of sorting them; the LSD passes + count_emit_kernel
 // stand behind as the device-flagged fallback (they return at once unless a leaf could not be counted).
@@ -843,9 +832,9 @@ int run_sort_count_leaves(kmcb200_ctx* ctx, Slot& s, uint64_t n_rec, uint32_t np
 	la.counter_max = ctx->prm.counter_max; la.counter_bytes = ctx->counter_bytes; la.suffix_bytes = ctx->suffix_bytes;
 	la.heavy_list = s.zero->heavy_list; la.heavy_count = &s.zero->heavy_count[0]; la.heavy_ticket = &s.zero->heavy_count[1]; la.heavy_cap = kHeavyListCap;
 	la.tmp = s.leaf_tmp; la.leaf_emit = s.leaf_emit; la.group_sum = s.zero->leaf_group_sum; la.lut = d_lut; la.result = d_result; la.ticket = &s.zero->msd_counters[3]; la.flags = flags;
-	if (int rc = DISPATCH_SLOTS(ctx, launch_leaves, WORDS, ctx, la, n_rec, st)) return rc;
+	if (int rc = launch_leaves<WORDS>(ctx, la, n_rec, st)) return rc;
 	if constexpr (WORDS == 1) {          // the large leaves the main launch only noted (none in a typical bin: the launch returns at once)
-		if (int rc = DISPATCH_SLOTS(ctx, launch_heavy_leaves, WORDS, ctx, la, st)) return rc;
+		if (int rc = launch_heavy_leaves(ctx, la, st)) return rc;
 	}
 	leaf_scan_kernel<<<(plan.n_leaves + 1023) / 1024, 1024, 0, st>>>(s.leaf_emit, s.zero->leaf_group_sum, plan.n_leaves, s.leaf_off, d_result, out_capacity, ob, flags, out_base);
 	leaf_gather_kernel<<<(plan.n_leaves + 7) / 8, 256, 0, st>>>(s.leaf_tmp, plan.start, s.leaf_emit, s.leaf_off, plan.n_leaves, ob, d_out, d_result, flags, out_base);
@@ -888,17 +877,8 @@ int run_bin(kmcb200_ctx* ctx, Slot& s, const uint8_t* d_bin, uint64_t size, uint
 	if (int rc = stage_expand(ctx, s, d_bin, size, n_rec, pack_bytes, n_packs, s.recs_a, st, em, packs_uploaded, d_lut, d_result, st_walk)) return rc;
 	CU(cudaEventRecord(s.ev_expand, st));
 	s.ran_expand = true;
-	bool in_b = false;
 	const uint32_t np_eff = (n_packs && pack_bytes) ? n_packs : 1u;
-	if (ctx->use_leaf) {
-		if (int rc = DISPATCH_WORDS(ctx, run_sort_count_leaves, ctx, s, n_rec, np_eff, d_out, out_capacity, d_lut, d_result, st, false, 0u, 0u, true)) return rc;
-	} else {
-		if (int rc = DISPATCH_WORDS(ctx, launch_sort, ctx, s, s.recs_a, s.recs_b, n_rec, ctx->key_bytes, 2u * ctx->prm.kmer_len, s.hist_mode, np_eff, st, &in_b)) return rc;
-		CU(cudaEventRecord(s.ev_sort, st));
-		s.ran_sort = true;
-		const void* sorted = in_b ? s.recs_b : s.recs_a;
-		if (int rc = stage_count(ctx, s, sorted, n_rec, d_out, out_capacity, d_lut, d_result, st, true, true)) return rc;
-	}
+	if (int rc = DISPATCH_WORDS(ctx, run_sort_count_leaves, ctx, s, n_rec, np_eff, d_out, out_capacity, d_lut, d_result, st, false, 0u, 0u, true)) return rc;
 	finish_result_kernel<<<1, 32, 0, st>>>(d_result, n_rec, s.zero->status, s.zero->msd_flags, host_result);
 	ctx->launches++;
 	CU(cudaEventRecord(s.ev_count, st));
@@ -1001,15 +981,7 @@ int bisect_blocks(kmcb200_ctx* ctx, const std::vector<uint64_t>& hist, uint32_t 
 int sort_count_block(kmcb200_ctx* ctx, Slot& s, void* region, void* rb, const KeyBlock& b, uint8_t* d_out, uint64_t out_capacity,
 	uint64_t* tot_lut, uint64_t* tot_res, const unsigned long long* appended, cudaStream_t st)
 {
-	const uint32_t k = ctx->prm.kmer_len;
-	if (ctx->use_leaf) {
-		if (int rc = DISPATCH_WORDS(ctx, run_sort_count_leaves, ctx, s, b.n, 1u, d_out, out_capacity, s.d_lut, s.d_result, st, true, b.bits, b.prefix, false, tot_res + 4, region, rb)) return rc;
-	} else {
-		bool in_b = false;
-		if (int rc = DISPATCH_WORDS(ctx, launch_sort, ctx, s, region, rb, b.n, ctx->key_bytes, 2u * k - b.bits, (int)kHistNone, 1u, st, &in_b)) return rc;
-		CU(cudaEventRecord(s.ev_sort, st));
-		if (int rc = stage_count(ctx, s, in_b ? rb : region, b.n, d_out, out_capacity, s.d_lut, s.d_result, st, false, false, tot_res + 4)) return rc;
-	}
+	if (int rc = DISPATCH_WORDS(ctx, run_sort_count_leaves, ctx, s, b.n, 1u, d_out, out_capacity, s.d_lut, s.d_result, st, true, b.bits, b.prefix, false, tot_res + 4, region, rb)) return rc;
 	accumulate_block_kernel<<<64, 256, 0, st>>>(tot_lut, s.d_lut, ctx->lut_entries, tot_res, s.d_result, appended, b.n);
 	ctx->launches++;
 	CU(cudaGetLastError());
@@ -1104,17 +1076,7 @@ int run_key_blocks(kmcb200_ctx* ctx, Slot& s, const std::vector<BinChunk>& chunk
 			if (int rc = stage_expand(ctx, s, s.d_bin + c.dev_off, c.bytes, kExpandUnknownRecs, pack_bytes + c.pack0, c.npacks, s.recs_a, st, ef)) return rc;
 		s.ran_expand = false;
 		CU(cudaEventRecord(s.ev_expand, st));
-		if (ctx->use_leaf) {
-			if (int rc = DISPATCH_WORDS(ctx, run_sort_count_leaves, ctx, s, b.n, 1u, d_out, out_capacity, s.d_lut, s.d_result, st, true, b.bits, b.prefix, false, tot_res + 4)) return rc;
-		} else {
-			bool in_b = false;
-			if (int rc = DISPATCH_WORDS(ctx, launch_sort, ctx, s, s.recs_a, s.recs_b, b.n, ctx->key_bytes, 2u * k - b.bits, (int)kHistNone, 1u, st, &in_b)) return rc;
-			CU(cudaEventRecord(s.ev_sort, st));
-			if (int rc = stage_count(ctx, s, in_b ? s.recs_b : s.recs_a, b.n, d_out, out_capacity, s.d_lut, s.d_result, st, false, false, tot_res + 4)) return rc;
-		}
-		accumulate_block_kernel<<<64, 256, 0, st>>>(tot_lut, s.d_lut, ctx->lut_entries, tot_res, s.d_result, s.d_out_counter, b.n);
-		ctx->launches++;
-		CU(cudaGetLastError());
+		if (int rc = sort_count_block(ctx, s, s.recs_a, s.recs_b, b, d_out, out_capacity, tot_lut, tot_res, s.d_out_counter, st)) return rc;
 	}
 	return 0;
 }
@@ -1211,10 +1173,8 @@ int kmcb200_create(const kmcb200_params* prm, kmcb200_ctx** out_ctx)
 	ctx->lut_entries = 1ull << (2 * prm->lut_prefix_len);
 	ctx->sm_count = dp.multiProcessorCount;
 	if (const char* e = getenv("KMCB200_SORT")) ctx->use_msd = std::string(e) != "lsd";
-	if (const char* e = getenv("KMCB200_LEAF")) ctx->use_leaf = std::string(e) != "sort";
 	if (const char* e = getenv("KMCB200_KEY_BLOCKS")) ctx->scatter_blocks = std::string(e) != "filter";
 	if (const char* e = getenv("KMCB200_KEY_BLOCK_RECORDS")) { const long long v = atoll(e); if (v >= 1024) ctx->key_block_records = (uint64_t)v; }
-	if (const char* e = getenv("KMCB200_OVERLAP_WALK")) ctx->overlap_walk = atoi(e) != 0;
 	{	// one sort needs two record buffers + the leaves' temporary records (8-byte padded) + ~2 bytes per record of tables: what 60 % of the
 		// free HBM (shared by the context's slots) can hold, below 2^32 records (32-bit record indices inside the kernels)
 		size_t free_b = 0, total_b = 0;
@@ -1232,16 +1192,13 @@ int kmcb200_create(const kmcb200_params* prm, kmcb200_ctx** out_ctx)
 		const std::string v(e);
 		if (v == "4:10" || v == "4:12") ctx->leaf_cta_slot_bits = atoi(v.c_str() + 2);
 	}
-	if (const char* e = getenv("KMCB200_LEAF_MAX_B2")) { const int v = atoi(e); if (v >= 8 && v <= 10) ctx->leaf_max_b2 = (uint32_t)v; }
-	if (const char* e = getenv("KMCB200_LEAF_TARGET")) { const int v = atoi(e); if (v >= 128 && v <= 8192) ctx->leaf_target = (uint32_t)v; }
 	if (const char* e = getenv("KMCB200_LEAF_FILL_PCT")) { const int v = atoi(e); if (v >= 10 && v <= 85) ctx->leaf_fill_pct = (uint32_t)v; }
 	if (const char* e = getenv("KMCB200_LEAF_RATIO0")) { const int v = atoi(e); if (v >= 8 && v <= 256) ctx->leaf_ratio0_q8 = (uint32_t)v; }
-	if (const char* e = getenv("KMCB200_LEAF_SLOT_BITS")) { const int b = atoi(e); if (b == 8 || b == 9 || b == 10) ctx->leaf_slot_bits = b; }
 	ctx->slots.resize(prm->n_slots);
 	auto bail = [&](int rc) { std::string e = ctx->err; kmcb200_destroy(ctx); g_create_error = e; return rc; };
 	if (cudaSetDevice(prm->device) != cudaSuccess) { ctx->err = "cudaSetDevice failed"; return bail(KMCB200_ERR_CUDA); }
 	if (int rc = DISPATCH_WORDS(ctx, setup_kernels, ctx)) return bail(rc);
-	if (int rc = DISPATCH_WORDS(ctx, setup_leaves_w, ctx)) return bail(rc);
+	if (int rc = DISPATCH_WORDS(ctx, setup_leaves, ctx)) return bail(rc);
 	if (cudaFuncSetAttribute(walk_packs_parallel_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kWalkChunk + 32) != cudaSuccess) {
 		ctx->err = "walk_packs_parallel_kernel setup failed"; return bail(KMCB200_ERR_CUDA);
 	}
@@ -1387,7 +1344,7 @@ static int submit_bin_impl(kmcb200_ctx* ctx, uint32_t slot, const uint8_t* super
 	CU(cudaEventRecord(s.ev_h2d, st));
 	CU(cudaStreamWaitEvent(ctx->compute, s.ev_h2d, 0));
 	if (int rc = run_bin(ctx, s, s.d_bin, size, n_rec, pack_bytes, n_packs, s.d_out, out_capacity, s.d_lut, s.d_result, ctx->compute, with_packs, s.h_result_dev,
-		ctx->overlap_walk ? st : nullptr)) return rc;
+		st)) return rc;
 	CU(cudaGetLastError());
 	CU(cudaEventRecord(s.ev_result, ctx->compute));
 	s.busy = true;

@@ -4,8 +4,8 @@ statistics).
     record per pack, empty packs; through every entry point (process_bin, two slots, the indexed form, dev_process_bin);
   * every record width (k = 5 .. 128, including k = 65 / 97 where the top symbols start a fresh word) against every counter width (0 .. 4
     bytes), through every leaf / sort variant, and counts that fill the third and fourth counter byte;
-  * the hybrid sort of wide records (KMCB200_LEAF=sort), the staged device calls (dev_expand -> dev_sort(hist_ready) -> dev_count) and the
-    knobs no other test sets."""
+  * the staged device calls (dev_expand -> dev_sort(hist_ready) -> dev_count), which sort the leaves of wide records, and the knobs no
+    other test sets."""
 import numpy as np
 import pytest
 
@@ -268,13 +268,13 @@ def test_oversized_bin_in_big_packs(oracle, monkeypatch, flow, target):
 K_P = {5: 1, 8: 4, 12: 4, 31: 7, 32: 4, 33: 5, 55: 7, 64: 8, 65: 5, 96: 8, 97: 5, 127: 11, 128: 8}
 WIDTHS = {"cw0": (1, 10 ** 9), "cw1": (255, 10 ** 9), "cw2": (65535, 10 ** 9), "cw3": (2 ** 24 - 1, 10 ** 9), "cw4": (2 ** 32 - 1, 10 ** 9),
           "cw1_by_cutoff_max": (2 ** 32 - 1, 200)}          # (counter_max, cutoff_max)
-KERNELS = {"default": {}, "leaf_sort": {"KMCB200_LEAF": "sort"}, "lsd": {"KMCB200_SORT": "lsd"}}
+KERNELS = {"default": {}, "lsd": {"KMCB200_SORT": "lsd"}}
 
 
 def width_matrix():
     """A fixed, seeded selection of (kernel, k, counter width, both_strands): every kernel meets every k once and every width at least twice.
-    The rows drawn second belonged to a retired leaf kernel.  They are still drawn, so that the other kernels' rows stay what they were, and
-    the oracle's corner test (test_oracle_golden) still takes their combinations."""
+    The rows drawn second and third belonged to retired leaf paths.  They are still drawn, so that the other kernels' rows stay what they
+    were, and the oracle's corner test (test_oracle_golden) still takes their combinations."""
     rng = np.random.default_rng(2026)
     names = list(WIDTHS)
     cases = []
@@ -337,7 +337,7 @@ def _dominant_bin(k, copies, seed):
     return pack_superkmers(k, lists)
 
 
-@pytest.mark.parametrize("kern", ["default", "leaf_sort", "lsd"])
+@pytest.mark.parametrize("kern", ["default", "lsd"])
 @pytest.mark.parametrize("k,copies,cntmax,fallback", [(31, 300_000, 2 ** 24 - 1, 0), (31, 300_000, 100_000, 0), (55, 100_000, 2 ** 24 - 1, 1), (65, 100_000, 70_000, 1)])
 def test_counts_in_the_third_counter_byte(oracle, monkeypatch, kern, k, copies, cntmax, fallback):
     """A k-mer with 10^5 .. 3 x 10^5 copies and 3-byte counters, unclamped or clamped between 2^16 and the count.  One-word records count it
@@ -377,54 +377,18 @@ def test_counts_in_the_fourth_counter_byte(oracle, cntmax):
     ctx.close()
 
 
-# ---------------------------------------------------------------------------------------------------------------------- LEAF=sort, wide records
-@pytest.mark.parametrize("k", [33, 55, 65, 97, 128])
-def test_leaf_sort_wide_records(oracle, monkeypatch, k):
-    """KMCB200_LEAF=sort with records of 2..4 words: the hybrid sort's msd_local_sort_kernel on key_bits = 2k (not a multiple of 8)."""
-    monkeypatch.setenv("KMCB200_LEAF", "sort")
-    p = Params(k=k, both_strands=k % 2 == 1, cutoff_min=1, lut_prefix_len=K_P[k])
-    b = synth_bin(60 + k, k, 9000, genome_len=20000, err=0.01)
-    assert b.n_rec >= 1 << 16
-    ctx = _ctx(p)
-    _same(ctx.process_bin(_skb(b)), oracle.process_bin(b, p))
-    assert "msd_local_sort" in ctx.stage_times()["pass_names"]
-    ctx.close()
-
-
-@pytest.mark.parametrize("flow", ["scatter", "filter"])
-@pytest.mark.parametrize("k", [55, 97])
-def test_leaf_sort_wide_records_in_key_blocks(oracle, monkeypatch, flow, k):
-    """... and an oversized bin with KMCB200_LEAF=sort: every key block is sorted (hybrid sort below the block's prefix bits) and counted by
-    count_emit_kernel, the branch of sort_count_block / run_key_blocks without leaf counting."""
-    monkeypatch.setenv("KMCB200_LEAF", "sort")
-    p = Params(k=k, cutoff_min=2, lut_prefix_len=K_P[k])
-    b = fast_bin(77 + k, k, 1_000_000)
-    e = oracle.process_bin(b, p)
-    ctx = _ctx(p)
-    l0 = ctx.kernel_launches()
-    _same(ctx.process_bin(_skb(b)), e)
-    l_one = ctx.kernel_launches() - l0
-    ctx.close()
-    monkeypatch.setenv("KMCB200_MAX_BLOCK_RECORDS", "150000")
-    monkeypatch.setenv("KMCB200_KEY_BLOCKS", flow)
-    ctx = _ctx(p)
-    l0 = ctx.kernel_launches()
-    _same(ctx.process_bin(_skb(b)), e)
-    assert ctx.kernel_launches() - l0 > 5 * l_one              # >= 7 key blocks, each a sort + count of its own
-    ctx.close()
-
-
 # ---------------------------------------------------------------------------------------------------------------------- staged device calls
-STAGED_CASES = [(n, k) for n in (20_000, 150_000) for k in (9, 31, 55, 128)]
+STAGED_CASES = [(n, k) for n in (20_000, 150_000) for k in (9, 31, 55, 128)] + [(150_000, k) for k in (33, 65, 97)]
 
 
 @pytest.mark.parametrize("n,k", STAGED_CASES, ids=["index-n%d-k%d" % c for c in STAGED_CASES])
 def test_staged_device_calls(oracle, n, k):
     """dev_expand -> dev_sort(hist_ready=True) -> dev_count: the sort takes the level-1 cells the expansion left (per expand tile); below
     2^16 records or k < 12 it is the plain LSD sort on the ZeroBlock the expansion zeroed.  The sorted records must be where dev_sort's
-    return value says."""
+    return value says.  Records of 2..4 words take msd_local_sort_kernel on key_bits = 2k (not a multiple of 8), including k = 33 / 65 /
+    97 where the top symbol starts a fresh word."""
     import torch
-    p = Params(k=k, both_strands=True, cutoff_min=2, lut_prefix_len=LAYOUT_P[k])
+    p = Params(k=k, both_strands=True, cutoff_min=2, lut_prefix_len=LAYOUT_P[k] if k in LAYOUT_P else K_P[k])
     b = fast_bin(4000 + k + n, k, n)
     exp_sorted = oracle.sort(oracle.expand(b, p), (k + 3) // 4)
     exp = oracle.compact(exp_sorted, p)
@@ -464,10 +428,9 @@ def test_staged_device_calls(oracle, n, k):
 
 
 # ---------------------------------------------------------------------------------------------------------------------- knobs
-def test_pipelined_slots_without_overlapped_walk(oracle, monkeypatch):
-    """KMCB200_OVERLAP_WALK=0: the index kernels of a submitted bin on the compute stream; bins of different sizes and pack layouts through
-    two slots (submit / wait), buffers reused and regrown."""
-    monkeypatch.setenv("KMCB200_OVERLAP_WALK", "0")
+def test_pipelined_slots_with_overlapped_walk(oracle):
+    """The index kernels of a submitted bin run on its slot's copy stream, next to the kernels of the bin before it on the compute stream;
+    bins of different sizes and pack layouts through two slots (submit / wait), buffers reused and regrown."""
     p = Params(k=31, cutoff_min=2, lut_prefix_len=7)
     ctx = _ctx(p, n_slots=2)
     bins = [synth_bin(100 + i, 31, n, genome_len=max(2000, n), err=0.01) for i, n in enumerate([3000, 50, 40000, 0, 7000, 1, 20000])]
@@ -508,17 +471,3 @@ def test_key_block_records(oracle, monkeypatch):
         ctx.close()
     assert launches["1024"] == launches[None]
     assert launches["20000"] - launches[None] >= 3 * 40
-
-
-def test_leaf_target_rule_picks_wide_second_level(monkeypatch):
-    """KMCB200_LEAF_TARGET / KMCB200_LEAF_MAX_B2 steer the default rule for the second partition level.  The rule only applies to bins of
-    more than 2^26 k-mers (below, ~1 K-record leaves need at most 8 bits whatever the target): the bin of the target workload's size
-    (1.2 x 10^8 k-mers) with leaves aimed at 128 records (10 bits) and 512 records (9 bits), against the unmodified reference's stored result."""
-    import test_gpu_parity as G
-    p, b = G.large_bin("large_second_level_k31")
-    for target, max_b2 in (("128", "10"), ("512", "9")):
-        monkeypatch.setenv("KMCB200_LEAF_TARGET", target)
-        monkeypatch.setenv("KMCB200_LEAF_MAX_B2", max_b2)
-        ctx = _ctx(p)
-        G._assert_reference(ctx.process_bin(b), b, "large_second_level_k31")
-        ctx.close()

@@ -31,10 +31,9 @@ def _check_bin(oracle, b: Bin, p: Params, ctx=None):
         ctx.close()
 
 
-@pytest.mark.parametrize("leaf", ["count", "sort"])
+@pytest.mark.parametrize("leaf", ["count"])
 @pytest.mark.parametrize("k,both,cmin", [(31, True, 2), (31, False, 1), (28, True, 1), (17, True, 1), (32, True, 2), (32, False, 1), (15, True, 1), (5, True, 1)])
-def test_bin_parity_one_word(oracle, monkeypatch, leaf, k, both, cmin):
-    monkeypatch.setenv("KMCB200_LEAF", leaf)
+def test_bin_parity_one_word(oracle, leaf, k, both, cmin):
     p = Params(k=k, both_strands=both, cutoff_min=cmin, lut_prefix_len=choose_lut_prefix_len(k))
     _check_bin(oracle, synth_bin(7, k, 20000, genome_len=30000, err=0.02), p)
 
@@ -55,18 +54,25 @@ def test_leaf_hash_cutoff_instances(oracle, k, both, cmin, cmax, cntmax):
     _check_bin(oracle, synth_bin(77 + k, k, 30000, genome_len=9000, err=0.01), p)
 
 
+LARGE_LEAVES = {"KMCB200_L2_BITS": "1", "KMCB200_LEAF_RATIO0": "8", "KMCB200_LEAF_KERNEL": "hash"}
+
+
 @pytest.mark.parametrize("env", [{"KMCB200_LEAF_FILL_PCT": "10"}, {"KMCB200_LEAF_RATIO0": "8"}, {"KMCB200_LEAF_RATIO0": "256", "KMCB200_LEAF_FILL_PCT": "85"},
-                                 {"KMCB200_L2_BITS": "2"}, {"KMCB200_L2_BITS": "2", "KMCB200_LEAF_RATIO0": "8", "KMCB200_LEAF_SLOT_BITS": "8"}])
+                                 {"KMCB200_L2_BITS": "2"}, LARGE_LEAVES])
 @pytest.mark.parametrize("coverage", ["30x", "distinct"])
 @pytest.mark.parametrize("k", [31, 55])
 def test_leaf_hash_round_planning(oracle, monkeypatch, env, coverage, k):
     """leaf_hash_kernel plans its table rounds from a running estimate of distinct k-mers per record: rounds planned far too small (many
-    predicated rounds over the leaf), far too large (the table fills up: the round is split on the next bit, binary descent), leaves of
-    ~10^4 records in 256-slot tables, duplicate-rich and all-distinct k-mers, one-word and two-word records (leaf_hash_wide_kernel)."""
+    predicated rounds over the leaf), far too large (the table fills up: the round is split on the next bit, binary descent), leaves
+    larger than the 1024-slot table (LARGE_LEAVES: bins twice as large in 512 leaves, mean leaves of ~1200 records at 30x and ~750
+    all-distinct ones: the all-distinct bin splits rounds in both record widths), duplicate-rich and all-distinct k-mers, one-word and
+    two-word records (leaf_hash_wide_kernel)."""
     for k_, v in env.items():
         monkeypatch.setenv(k_, v)
     p = Params(k=k, cutoff_min=2 if coverage == "30x" else 1, lut_prefix_len=7)
-    b = synth_bin(5, k, 26000, genome_len=10000, err=0.01) if coverage == "30x" else synth_bin(6, k, 16000, genome_len=4000000, err=0.0)
+    scale = 2 if env is LARGE_LEAVES else 1
+    b = (synth_bin(5, k, 26000 * scale, genome_len=10000 * scale, err=0.01) if coverage == "30x"
+         else synth_bin(6, k, 16000 * scale, genome_len=4000000 * scale, err=0.0))
     _check_bin(oracle, b, p)
 
 
@@ -85,12 +91,11 @@ def test_bin_parity_multi_word(oracle, k, both, cmin):
     _check_bin(oracle, synth_bin(11, k, 8000, genome_len=12000, err=0.02), p)
 
 
-@pytest.mark.parametrize("slot_bits", [8, 9, 10])
+@pytest.mark.parametrize("slot_bits", [10])
 @pytest.mark.parametrize("k,both,cmin,p_len", [(31, True, 2, 7), (55, True, 2, 7), (55, False, 1, 3), (33, True, 1, 5), (64, True, 2, 8), (70, True, 1, 6),
                                                (96, False, 2, 8), (128, True, 1, 8), (32, False, 1, 4), (17, True, 1, 5)])
-def test_leaf_path_all_widths(oracle, monkeypatch, slot_bits, k, both, cmin, p_len):
-    """~170 K k-mers (the hybrid MSD path + warp-counted leaves) for every record width and every table size."""
-    monkeypatch.setenv("KMCB200_LEAF_SLOT_BITS", str(slot_bits))
+def test_leaf_path_all_widths(oracle, slot_bits, k, both, cmin, p_len):
+    """~170 K k-mers (the hybrid MSD path + warp-counted leaves, 2^slot_bits slots per warp table) for every record width."""
     p = Params(k=k, both_strands=both, cutoff_min=cmin, lut_prefix_len=p_len)
     _check_bin(oracle, synth_bin(31 + k, k, 14000, genome_len=9000, err=0.01), p)
 
@@ -383,9 +388,9 @@ def test_benchmark_scale_bit_exact_vs_reference(k, p_len):
 
 def test_large_second_level_bit_exact_vs_reference(monkeypatch):
     """A bin of the target workload's size (1.2e8 k-mers) against the reference: the default second partition level (8 bits, leaves of
-    ~1.8 K records) and a forced 9-bit one (512-digit count and scatter, 2^17 leaves)."""
+    ~1.8 K records) and forced 9- and 10-bit ones (512- and 1024-digit count and scatter, 2^17 and 2^18 leaves)."""
     p, b = large_bin("large_second_level_k31")
-    for bits in (None, "9"):
+    for bits in (None, "9", "10"):
         if bits:
             monkeypatch.setenv("KMCB200_L2_BITS", bits)
         ctx = _ctx(p)

@@ -221,34 +221,30 @@ class BinResult:
         return (self.n_unique, self.n_cutoff_min, self.n_cutoff_max, self.n_total)
 
 
-class Stage2Context:
-    """One GPU's stage-2 engine (one per sorter thread in KMC terms)."""
+class _Handle:
+    """One handle of the C ABI: the symbols <_prefix>_<_create> / _destroy / _last_error, create-or-raise, error check, close."""
+    _prefix = None
+    _create = "create"
 
-    def __init__(self, params: Stage2Params, device=0, n_slots=1):
+    def _sym(self, name):
+        return getattr(self.lib, "%s_%s" % (self._prefix, name))
+
+    def _open(self, *args):
+        """The family's create call on `args`; its handle pointer is the last argument."""
         self.lib = load_library()
-        self.params = params
         self._h = C.c_void_p(None)
-        p = _Params(params.kmer_len, int(params.both_strands), params.cutoff_min, min(params.cutoff_max, 0xFFFFFFFF),
-                    min(params.counter_max, 0xFFFFFFFF), params.lut_prefix_len, device, n_slots)
-        rc = self.lib.kmcb200_create(C.byref(p), C.byref(self._h))
+        rc = self._sym(self._create)(*args, C.byref(self._h))
         if rc != 0:
-            raise KmcB200Error(rc, (self.lib.kmcb200_last_error(None) or b"").decode())
-        self.device = device
-        self.n_slots = n_slots
-        self.words = (params.kmer_len + 31) // 32
-        self.key_bytes = (params.kmer_len + 3) // 4
-        self.out_rec_bytes = self.lib.kmcb200_out_rec_bytes(self._h)
-        self.lut_entries = self.lib.kmcb200_lut_entries(self._h)
+            raise KmcB200Error(rc, (self._sym("last_error")(None) or b"").decode())
 
-    # -- plumbing
     def _check(self, rc):
         if rc < 0:
-            raise KmcB200Error(rc, (self.lib.kmcb200_last_error(self._h) or b"").decode())
+            raise KmcB200Error(rc, (self._sym("last_error")(self._h) or b"").decode())
         return rc
 
     def close(self):
         if self._h:
-            self.lib.kmcb200_destroy(self._h)
+            self._sym("destroy")(self._h)
             self._h = C.c_void_p(None)
 
     def __del__(self):
@@ -256,6 +252,23 @@ class Stage2Context:
             self.close()
         except Exception:
             pass
+
+
+class Stage2Context(_Handle):
+    """One GPU's stage-2 engine (one per sorter thread in KMC terms)."""
+    _prefix = "kmcb200"
+
+    def __init__(self, params: Stage2Params, device=0, n_slots=1):
+        self.params = params
+        p = _Params(params.kmer_len, int(params.both_strands), params.cutoff_min, min(params.cutoff_max, 0xFFFFFFFF),
+                    min(params.counter_max, 0xFFFFFFFF), params.lut_prefix_len, device, n_slots)
+        self._open(C.byref(p))
+        self.device = device
+        self.n_slots = n_slots
+        self.words = (params.kmer_len + 31) // 32
+        self.key_bytes = (params.kmer_len + 3) // 4
+        self.out_rec_bytes = self.lib.kmcb200_out_rec_bytes(self._h)
+        self.lut_entries = self.lib.kmcb200_lut_entries(self._h)
 
     def out_capacity(self, n_rec):
         return int(self.lib.kmcb200_out_capacity(self._h, n_rec))
@@ -351,21 +364,15 @@ class Stage2Context:
         self._check(self.lib.kmcb200_dev_count(self._h, slot, d_sorted, n, d_out, out_capacity, d_lut, d_result, stream))
 
 
-class DbWriter:
+class DbWriter(_Handle):
     """KMC database files from per-bin results (kmcb200_db_*): pinned staging ring + writer thread; format of kb_completer.cpp:59-326."""
+    _prefix = "kmcb200_db"
+    _create = "open"
 
     def __init__(self, path_prefix, kmer_len, counter_size, lut_prefix_len, signature_len, cutoff_min, cutoff_max, both_strands, staging_bytes=1 << 28):
-        self.lib = load_library()
-        self._h = C.c_void_p(None)
         p = _DbParams(kmer_len, counter_size, lut_prefix_len, signature_len, cutoff_min, min(cutoff_max, 0xFFFFFFFF), int(both_strands))
-        rc = self.lib.kmcb200_db_open(C.byref(p), path_prefix.encode(), staging_bytes, C.byref(self._h))
-        if rc != 0:
-            raise KmcB200Error(rc, (self.lib.kmcb200_db_last_error(None) or b"").decode())
+        self._open(C.byref(p), path_prefix.encode(), staging_bytes)
         self.lut_entries = 1 << (2 * lut_prefix_len)
-
-    def _check(self, rc):
-        if rc != 0:
-            raise KmcB200Error(rc, (self.lib.kmcb200_db_last_error(self._h) or b"").decode())
 
     @property
     def records(self):
@@ -391,43 +398,27 @@ class DbWriter:
             raise KmcB200Error(rc, "kmcb200_db_close")
         return tuple(int(x) for x in tot)
 
+    def __del__(self):          # only close() ends a database: a writer that is dropped leaves its files unfinished
+        pass
 
-class Splitter:
+
+class Splitter(_Handle):
     """Stage 1 on one GPU (kmcb200_splitter_*): batches of sequences -> KMC bins (CSplitter::ProcessReads, kmc_core/splitter.cpp:557-677).
 
     A batch is one byte array in which every byte other than ACGTacgt separates (reads.sequences_to_batch makes one from FASTQ / FASTA).
     `signature_map` has 4^signature_len + 1 entries, each below n_bins."""
+    _prefix = "kmcb200_splitter"
 
     def __init__(self, kmer_len, signature_len, signature_map, n_bins=None, device=0, max_batch_bytes=1 << 26):
-        self.lib = load_library()
         sig_map = np.ascontiguousarray(signature_map, dtype=np.uint32)
         if sig_map.size != (1 << (2 * signature_len)) + 1:
             raise KmcB200Error(ERR_INVALID, "signature_map has %d entries, 4^%d + 1 expected" % (sig_map.size, signature_len))
         self.n_bins = int(sig_map.max()) + 1 if n_bins is None else int(n_bins)
         self.kmer_len, self.signature_len, self.max_batch_bytes = kmer_len, signature_len, max_batch_bytes
-        self._h = C.c_void_p(None)
         p = _SplitParams(kmer_len, signature_len, self.n_bins, device, max_batch_bytes)
-        rc = self.lib.kmcb200_splitter_create(C.byref(p), sig_map.ctypes.data, C.byref(self._h))
-        if rc != 0:
-            raise KmcB200Error(rc, (self.lib.kmcb200_splitter_last_error(None) or b"").decode())
+        self._open(C.byref(p), sig_map.ctypes.data)
         self._out = np.empty(0, dtype=np.uint8)
         self._packs = np.empty(0, dtype=np.uint64)
-
-    def _check(self, rc):
-        if rc < 0:
-            raise KmcB200Error(rc, (self.lib.kmcb200_splitter_last_error(self._h) or b"").decode())
-        return rc
-
-    def close(self):
-        if self._h:
-            self.lib.kmcb200_splitter_destroy(self._h)
-            self._h = C.c_void_p(None)
-
-    def __del__(self):
-        try:
-            self.close()
-        except Exception:
-            pass
 
     def kernel_launches(self):
         return int(self.lib.kmcb200_splitter_kernel_launches(self._h))
@@ -494,34 +485,15 @@ class Splitter:
         return out
 
 
-class SignatureStats:
+class SignatureStats(_Handle):
     """Stage 0 on one GPU (kmcb200_sigstats_*): k-mers per signature over batches of sequences, what CSplitter::CalcStats counts
     (kmc_core/splitter.cpp:439-533).  Batches as for Splitter; the counts (uint32[4^signature_len + 1]) add up until reset()."""
+    _prefix = "kmcb200_sigstats"
 
     def __init__(self, kmer_len, signature_len, device=0, max_batch_bytes=1 << 26):
-        self.lib = load_library()
         self.kmer_len, self.signature_len, self.max_batch_bytes = kmer_len, signature_len, max_batch_bytes
-        self._h = C.c_void_p(None)
         p = _SigstatsParams(kmer_len, signature_len, device, 0, max_batch_bytes)
-        rc = self.lib.kmcb200_sigstats_create(C.byref(p), C.byref(self._h))
-        if rc != 0:
-            raise KmcB200Error(rc, (self.lib.kmcb200_sigstats_last_error(None) or b"").decode())
-
-    def _check(self, rc):
-        if rc < 0:
-            raise KmcB200Error(rc, (self.lib.kmcb200_sigstats_last_error(self._h) or b"").decode())
-        return rc
-
-    def close(self):
-        if self._h:
-            self.lib.kmcb200_sigstats_destroy(self._h)
-            self._h = C.c_void_p(None)
-
-    def __del__(self):
-        try:
-            self.close()
-        except Exception:
-            pass
+        self._open(C.byref(p))
 
     def kernel_launches(self):
         return int(self.lib.kmcb200_sigstats_kernel_launches(self._h))
@@ -552,36 +524,17 @@ class SignatureStats:
         self._check(self.lib.kmcb200_sigstats_reset(self._h))
 
 
-class SmallKCounter:
+class SmallKCounter(_Handle):
     """Small k (1..13) on one GPU (kmcb200_smallk_*), KMC's small-k mode (kmc_core/kmc.h:677-960): every k-mer of the batches counted in
     a direct array of 4^k uint64 counters (CSplitter::ProcessReadsSmallK), then a KMC1-format database (CSmallKCompleter).  Batches as for
     Splitter; the counts add up until reset().  There are no bins, so no signature length, map or caller-chosen LUT prefix length: finish()
     picks the LUT prefix length as the reference does."""
+    _prefix = "kmcb200_smallk"
 
     def __init__(self, kmer_len, both_strands=True, device=0, max_batch_bytes=1 << 26):
-        self.lib = load_library()
         self.kmer_len, self.both_strands, self.max_batch_bytes = kmer_len, bool(both_strands), max_batch_bytes
-        self._h = C.c_void_p(None)
         p = _SmallKParams(kmer_len, int(bool(both_strands)), device, 0, max_batch_bytes)
-        rc = self.lib.kmcb200_smallk_create(C.byref(p), C.byref(self._h))
-        if rc != 0:
-            raise KmcB200Error(rc, (self.lib.kmcb200_smallk_last_error(None) or b"").decode())
-
-    def _check(self, rc):
-        if rc < 0:
-            raise KmcB200Error(rc, (self.lib.kmcb200_smallk_last_error(self._h) or b"").decode())
-        return rc
-
-    def close(self):
-        if self._h:
-            self.lib.kmcb200_smallk_destroy(self._h)
-            self._h = C.c_void_p(None)
-
-    def __del__(self):
-        try:
-            self.close()
-        except Exception:
-            pass
+        self._open(C.byref(p))
 
     def kernel_launches(self):
         return int(self.lib.kmcb200_smallk_kernel_launches(self._h))
@@ -643,7 +596,7 @@ def _as_u8(raw):
     return np.ascontiguousarray(np.frombuffer(raw, dtype=np.uint8) if isinstance(raw, (bytes, bytearray, memoryview)) else raw, dtype=np.uint8)
 
 
-class FastxParser:
+class FastxParser(_Handle):
     """Reads text -> batch on one GPU (kmcb200_fastx_*): raw FASTQ or FASTA chunks become the batches Splitter and SignatureStats take,
     byte for byte what kmc_b200.reads.sequences_to_batch makes of the whole file.  `fmt` is FASTQ / FASTA (or "fastq" / "fasta"): the
     caller's choice, by the first byte of the file's first non-empty line.
@@ -652,32 +605,13 @@ class FastxParser:
     next chunk must start.  A record longer than the chunk is an error: since the limit here is raw bytes per chunk, a FASTQ record of more
     than about max_chunk_bytes / 2 bases cannot be parsed, where the host path (sequences_to_batch + batches) accepts sequences up to the
     batch size."""
+    _prefix = "kmcb200_fastx"
 
     def __init__(self, fmt, device=0, max_chunk_bytes=1 << 26):
-        self.lib = load_library()
         self.format = {"fastq": FASTQ, "fasta": FASTA}.get(fmt, fmt) if isinstance(fmt, str) else int(fmt)
         self.max_chunk_bytes = max_chunk_bytes
-        self._h = C.c_void_p(None)
         p = _FastxParams(device, self.format, max_chunk_bytes)
-        rc = self.lib.kmcb200_fastx_create(C.byref(p), C.byref(self._h))
-        if rc != 0:
-            raise KmcB200Error(rc, (self.lib.kmcb200_fastx_last_error(None) or b"").decode())
-
-    def _check(self, rc):
-        if rc < 0:
-            raise KmcB200Error(rc, (self.lib.kmcb200_fastx_last_error(self._h) or b"").decode())
-        return rc
-
-    def close(self):
-        if self._h:
-            self.lib.kmcb200_fastx_destroy(self._h)
-            self._h = C.c_void_p(None)
-
-    def __del__(self):
-        try:
-            self.close()
-        except Exception:
-            pass
+        self._open(C.byref(p))
 
     def kernel_launches(self):
         return int(self.lib.kmcb200_fastx_kernel_launches(self._h))

@@ -31,6 +31,8 @@
 
 using namespace kmcb;
 
+#include "host_support.inl"
+
 namespace {
 
 constexpr int kMaxPasses = 4 * 8;                 // key bytes of a 4-word record
@@ -66,46 +68,41 @@ static_assert(sizeof(ZeroBlock) % 4 == 0, "zeroed word by word");
 struct Slot {
 	cudaStream_t stream = nullptr;
 	// records
-	uint8_t* recs_a = nullptr; size_t recs_a_cap = 0;
-	uint8_t* recs_b = nullptr; size_t recs_b_cap = 0;
-	uint8_t* recs_x = nullptr; size_t recs_x_cap = 0;        // kmcb200_process_bin_multi: this GPU's key range, gathered from all GPUs
-	// bin + index
-	uint8_t* d_bin = nullptr; size_t bin_cap = 0;
-	uint64_t* d_pack_start = nullptr; size_t packs_cap = 0;
-	uint64_t* h_pack_start[kStageRing] = {}; cudaEvent_t ev_pack[kStageRing] = {}; int ring = 0;   // pinned staging of the pack offsets
-	uint32_t* pack_nsk = nullptr; uint32_t* pack_nk = nullptr; uint32_t* pack_tbase = nullptr; uint64_t* pack_kbase = nullptr;
-	uint32_t* pack_done = nullptr;
-	uint32_t* sk_off = nullptr; size_t sk_off_cap = 0;
-	uint32_t* sk_kpre = nullptr; size_t sk_kpre_cap = 0;
-	uint32_t* tile_first = nullptr; size_t tile_first_cap = 0;
-	uint32_t* tile_pack = nullptr; size_t tile_pack_cap = 0;
-	uint4* tile_desc = nullptr; size_t tile_desc_cap = 0;
-	ZeroBlock* zero = nullptr;
-	uint64_t* desc = nullptr; size_t desc_cap = 0;          // radix look-back descriptors
+	DevBuf<uint8_t> recs_a, recs_b;
+	DevBuf<uint8_t> recs_x;                                 // kmcb200_process_bin_multi: this GPU's key range, gathered from all GPUs
+	// bin + index (the pack tables are allocated together, d_pack_start last: its capacity is theirs)
+	DevBuf<uint8_t> d_bin;
+	DevBuf<uint64_t> d_pack_start;
+	PinnedBuf<uint64_t> h_pack_start[kStageRing]; cudaEvent_t ev_pack[kStageRing] = {}; int ring = 0;   // pinned staging of the pack offsets
+	DevBuf<uint32_t> pack_nsk, pack_nk, pack_tbase, pack_done; DevBuf<uint64_t> pack_kbase;
+	DevBuf<uint32_t> sk_off, sk_kpre, tile_first, tile_pack;
+	DevBuf<uint4> tile_desc;
+	DevBuf<ZeroBlock> zero;
+	DevBuf<uint64_t> desc;                                  // radix look-back descriptors
 	// hybrid MSD sort: bucket boundaries and work-item tables
-	uint64_t* msd_seg1 = nullptr;                           // [2]      {0, n}
-	uint64_t* msd_start2 = nullptr;                         // [257]    level-1 buckets
-	uint64_t* msd_start3 = nullptr;                         // [kMaxLeaves + 1]  level-2 buckets
-	uint32_t* msd_item_base1 = nullptr;                     // [2]
-	uint32_t* msd_item_base2 = nullptr;                     // [257]
-	uint32_t* msd_item_seg2 = nullptr; size_t msd_item_seg2_cap = 0;
-	uint64_t* msd_item_lo1 = nullptr; size_t msd_item_lo1_cap = 0;      // level-1 items = expand tiles
-	uint16_t* msd_item_cnt1 = nullptr; size_t msd_item_cnt1_cap = 0;
-	uint16_t* msd_cells = nullptr; size_t msd_cells_cap = 0;            // counts[segment][digit][item] (level 1, then reused by level 2)
-	uint32_t* msd_cell_scan = nullptr; size_t msd_cell_scan_cap = 0;    // their exclusive scan
-	uint32_t* msd_block_sums = nullptr; size_t msd_block_sums_cap = 0;
+	DevBuf<uint64_t> msd_seg1;                              // [2]      {0, n}
+	DevBuf<uint64_t> msd_start2;                            // [257]    level-1 buckets
+	DevBuf<uint64_t> msd_start3;                            // [kMaxLeaves + 1]  level-2 buckets
+	DevBuf<uint32_t> msd_item_base1;                        // [2]
+	DevBuf<uint32_t> msd_item_base2;                        // [257]
+	DevBuf<uint32_t> msd_item_seg2;
+	DevBuf<uint64_t> msd_item_lo1;                          // level-1 items = expand tiles
+	DevBuf<uint16_t> msd_item_cnt1;
+	DevBuf<uint16_t> msd_cells;                             // counts[segment][digit][item] (level 1, then reused by level 2)
+	DevBuf<uint32_t> msd_cell_scan;                         // their exclusive scan
+	DevBuf<uint32_t> msd_block_sums;
 	// leaf-count path
-	uint8_t* leaf_tmp = nullptr; size_t leaf_tmp_cap = 0;
-	uint32_t* leaf_emit = nullptr; uint64_t* leaf_off = nullptr;          // [kMaxLeaves]
+	DevBuf<uint8_t> leaf_tmp;
+	DevBuf<uint32_t> leaf_emit; DevBuf<uint64_t> leaf_off;  // [kMaxLeaves]
 	const char* pass_names[kMaxPasses + 8] = {};
 	uint32_t last_n_packs = 1;
-	uint64_t* cdesc = nullptr; size_t cdesc_cap = 0;        // count look-back descriptors
+	DevBuf<uint64_t> cdesc;                                 // count look-back descriptors
 	int hist_mode = 0;                                      // what the last expansion left for the sort: kHistNone / kHistTiles / kHistTotals
 	ExpandArgs expand_args{};                               // kHistTotals: the index's arguments, for the level-1 partition expansion
 	// outputs of the host-buffer path
-	uint8_t* d_out = nullptr; size_t out_cap = 0;
-	uint64_t* d_lut = nullptr;
-	uint64_t* d_result = nullptr; uint64_t* h_result = nullptr; uint64_t* h_result_dev = nullptr;
+	DevBuf<uint8_t> d_out;
+	DevBuf<uint64_t> d_lut;
+	DevBuf<uint64_t> d_result; PinnedBuf<uint64_t> h_result; uint64_t* h_result_dev = nullptr;      // (h_result as the device sees it)
 	// events
 	cudaEvent_t ev_begin = nullptr, ev_expand = nullptr, ev_sort = nullptr, ev_count = nullptr, ev_result = nullptr;
 	cudaEvent_t ev_h2d = nullptr, ev_done = nullptr, ev_walk = nullptr;           // copy stream <-> compute stream hand-over
@@ -113,12 +110,12 @@ struct Slot {
 	int n_passes_run = 0;                                   // number of timed sort intervals (ev_pass[i] .. ev_pass[i+1])
 	bool ran_expand = false, ran_sort = false, ran_count = false;
 	// oversized bins
-	uint64_t* d_hist12 = nullptr; unsigned long long* d_out_counter = nullptr; size_t out_counter_cap = 0;
-	uint16_t* d_blk_of_prefix = nullptr; uint64_t* d_region_start = nullptr; size_t region_cap = 0; bool last_scatter = false;      // key blocks, scatter flow
-	uint64_t* tot_lut = nullptr; uint64_t* tot_res = nullptr; uint32_t last_blocks = 0;      // totals over the key blocks
+	DevBuf<uint64_t> d_hist12; DevBuf<unsigned long long> d_out_counter;
+	DevBuf<uint16_t> d_blk_of_prefix; DevBuf<uint64_t> d_region_start;                        // key blocks, scatter flow
+	DevBuf<uint64_t> tot_lut, tot_res;                                                        // totals over the key blocks
 	bool scan_lut = false; uint64_t scan_base = 0;                                            // kmcb200_wait_bin_scanned
-	uint8_t* d_extras = nullptr; size_t extras_cap = 0; uint64_t* d_pack_rec = nullptr; size_t pack_rec_cap = 0;      // kmcb200_submit_bin_indexed (N4)
-	uint64_t* h_pack_rec = nullptr; size_t h_pack_rec_cap = 0; bool have_extras = false;
+	DevBuf<uint8_t> d_extras; DevBuf<uint64_t> d_pack_rec;                                    // kmcb200_submit_bin_indexed (N4)
+	PinnedBuf<uint64_t> h_pack_rec; bool have_extras = false;
 	bool sync_done = false; uint64_t sync_out_bytes = 0; uint64_t sync_stats[4] = {};
 	// pending host-buffer bin
 	bool busy = false;
@@ -127,7 +124,8 @@ struct Slot {
 
 }  // namespace
 
-struct kmcb200_ctx {
+struct kmcb200_ctx : HandleBase {
+	static std::string& create_error() { return g_create_error; }
 	kmcb200_params prm{};
 	int words = 1;
 	uint32_t key_bytes = 0, suffix_bytes = 0, counter_bytes = 0;
@@ -148,34 +146,14 @@ struct kmcb200_ctx {
 	uint64_t max_block_records = 1ull << 28;                // a bin with more k-mers is counted key block by key block: from the free HBM at create (KMCB200_MAX_BLOCK_RECORDS overrides)
 	uint64_t max_chunk_bytes = 1ull << 30;                  // KMCB200_MAX_CHUNK_BYTES: ... and expanded chunk by chunk
 	uint32_t epoch = 1;
-	uint64_t launches = 0;
 	// All kernels of a context run on ONE stream: the persistent radix passes size their grids to fill the GPU and two of
 	// them side by side only steal SMs from each other.  The slots' own streams carry the
 	// host<->device copies, so the copies of one bin overlap the kernels of another.
 	cudaStream_t compute = nullptr;
 	std::vector<Slot> slots;
-	std::string err;
 };
 
 namespace {
-
-int fail(kmcb200_ctx* c, int code, const char* fmt, ...)
-{
-	char buf[512];
-	va_list ap;
-	va_start(ap, fmt);
-	vsnprintf(buf, sizeof buf, fmt, ap);
-	va_end(ap);
-	if (c) c->err = buf;
-	else g_create_error = buf;
-	return code;
-}
-
-#define CU(call)                                                                                             \
-	do {                                                                                                     \
-		cudaError_t e_ = (call);                                                                             \
-		if (e_ != cudaSuccess) return fail(ctx, KMCB200_ERR_CUDA, "%s failed: %s (%s:%d)", #call, cudaGetErrorString(e_), __FILE__, __LINE__); \
-	} while (0)
 
 // Zeroing on the compute stream is done by a kernel, not by cudaMemsetAsync: a memset may be carried out by a copy engine, and
 // the copy engines are busy with the next bin's 66 MB host-to-device transfer - the kernels behind the memset would wait for it.
@@ -186,11 +164,11 @@ __global__ void zero_words_kernel(uint32_t* p, size_t n_words)
 int zero_async(kmcb200_ctx* ctx, void* ptr, size_t bytes, cudaStream_t st)
 {
 	if (bytes == 0) return 0;
-	if ((reinterpret_cast<uintptr_t>(ptr) & 3u) || (bytes & 3u) || bytes > (size_t(1) << 28)) { CU(cudaMemsetAsync(ptr, 0, bytes, st)); return 0; }
+	if ((reinterpret_cast<uintptr_t>(ptr) & 3u) || (bytes & 3u) || bytes > (size_t(1) << 28)) { CU(ctx, cudaMemsetAsync(ptr, 0, bytes, st)); return 0; }
 	const size_t n = bytes / 4;
 	zero_words_kernel<<<(unsigned)std::min<size_t>((n + 255) / 256, 1184), 256, 0, st>>>(reinterpret_cast<uint32_t*>(ptr), n);
 	ctx->launches++;
-	CU(cudaGetLastError());
+	CU(ctx, cudaGetLastError());
 	return 0;
 }
 
@@ -203,31 +181,19 @@ __global__ void bin_init_kernel(uint32_t* zero_block, uint32_t zero_words, uint3
 	if (result && i0 < 16) result[i0] = 0u;
 }
 
-uint32_t byte_log(uint64_t x) { return x < (1u << 8) ? 1 : x < (1u << 16) ? 2 : x < (1u << 24) ? 3 : 4; }   // defs.h:121
-
-template <typename T>
-int ensure(kmcb200_ctx* ctx, T*& p, size_t& cap, size_t need_elems, bool zero = false)
-{
-	if (need_elems <= cap && p) return 0;
-	size_t n = std::max<size_t>(need_elems + need_elems / 8, 1024);
-	if (p) CU(cudaFree(p));
-	p = nullptr; cap = 0;
-	CU(cudaMalloc(reinterpret_cast<void**>(&p), n * sizeof(T) + 256));
-	if (zero) { CU(cudaMemset(p, 0, n * sizeof(T) + 256)); CU(cudaDeviceSynchronize()); }   // the slot streams are non-blocking
-	cap = n;
-	return 0;
-}
+constexpr Slack kSlotSlack{8, 1024, 256};         // a slot's per-bin buffers: an eighth more than the bin needs
+constexpr Slack kBlockTableSlack{0, 64, 0};       // per-key-block tables of an oversized bin
 
 // `count` consecutive epochs for the look-back descriptors of the next launches
 int next_epoch(kmcb200_ctx* ctx, uint32_t* out, uint32_t count = 1)
 {
 	if (ctx->epoch + count >= kEpochLimit) {   // wrap: forget every descriptor ever written - but only once nothing is spinning on them any more
-		CU(cudaDeviceSynchronize());
+		CU(ctx, cudaDeviceSynchronize());
 		for (auto& s : ctx->slots) {
-			if (s.desc) CU(cudaMemset(s.desc, 0, s.desc_cap * sizeof(uint64_t)));
-			if (s.cdesc) CU(cudaMemset(s.cdesc, 0, s.cdesc_cap * sizeof(uint64_t)));
+			if (s.desc) CU(ctx, cudaMemset(s.desc, 0, s.desc.cap * sizeof(uint64_t)));
+			if (s.cdesc) CU(ctx, cudaMemset(s.cdesc, 0, s.cdesc.cap * sizeof(uint64_t)));
 		}
-		CU(cudaDeviceSynchronize());
+		CU(ctx, cudaDeviceSynchronize());
 		ctx->epoch = 1;
 	}
 	*out = ctx->epoch;
@@ -239,22 +205,22 @@ int next_epoch(kmcb200_ctx* ctx, uint32_t* out, uint32_t count = 1)
 template <int WORDS>
 int setup_kernels(kmcb200_ctx* ctx)
 {
-	CU(cudaFuncSetAttribute(radix_pass_kernel<WORDS>, cudaFuncAttributeMaxDynamicSharedMemorySize, SortSmem<WORDS>::kBytes));
-	CU(cudaFuncSetAttribute(lsd_sort_kernel<WORDS>, cudaFuncAttributeMaxDynamicSharedMemorySize, SortSmem<WORDS>::kBytes));
-	CU(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&ctx->occ_radix, lsd_sort_kernel<WORDS>, SortCfg<WORDS>::kThreads, SortSmem<WORDS>::kBytes));
-	CU(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&ctx->occ_expand, expand_kernel<WORDS>, ExpandCfg<WORDS>::kThreads, 0));
+	CU(ctx, cudaFuncSetAttribute(radix_pass_kernel<WORDS>, cudaFuncAttributeMaxDynamicSharedMemorySize, SortSmem<WORDS>::kBytes));
+	CU(ctx, cudaFuncSetAttribute(lsd_sort_kernel<WORDS>, cudaFuncAttributeMaxDynamicSharedMemorySize, SortSmem<WORDS>::kBytes));
+	CU(ctx, cudaOccupancyMaxActiveBlocksPerMultiprocessor(&ctx->occ_radix, lsd_sort_kernel<WORDS>, SortCfg<WORDS>::kThreads, SortSmem<WORDS>::kBytes));
+	CU(ctx, cudaOccupancyMaxActiveBlocksPerMultiprocessor(&ctx->occ_expand, expand_kernel<WORDS>, ExpandCfg<WORDS>::kThreads, 0));
 	if constexpr (expand_partition_supported<WORDS>())
-		CU((cudaOccupancyMaxActiveBlocksPerMultiprocessor(&ctx->occ_expand_part, expand_kernel<WORDS, kExpandPartition>, ExpandCfg<WORDS>::kThreads, 0)));
+		CU(ctx, (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&ctx->occ_expand_part, expand_kernel<WORDS, kExpandPartition>, ExpandCfg<WORDS>::kThreads, 0)));
 	const size_t cs = count_smem_bytes<WORDS>(ctx->suffix_bytes + ctx->counter_bytes);
-	CU(cudaFuncSetAttribute(count_emit_kernel<WORDS>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)cs));
-	CU(cudaFuncSetAttribute(msd_partition_kernel<WORDS>, cudaFuncAttributeMaxDynamicSharedMemorySize, MsdSmem<WORDS>::kBytes));
-	CU(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&ctx->occ_msd_part, msd_partition_kernel<WORDS>, MsdCfg<WORDS>::kThreads + 32, MsdSmem<WORDS>::kBytes));
-	CU(cudaFuncSetAttribute(msd_partition_kernel<WORDS, 1024>, cudaFuncAttributeMaxDynamicSharedMemorySize, MsdSmem<WORDS, 1024>::kBytes));
-	CU(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&ctx->occ_msd_part_wide, msd_partition_kernel<WORDS, 1024>, MsdCfg<WORDS>::kThreads + 32, MsdSmem<WORDS, 1024>::kBytes));
+	CU(ctx, cudaFuncSetAttribute(count_emit_kernel<WORDS>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)cs));
+	CU(ctx, cudaFuncSetAttribute(msd_partition_kernel<WORDS>, cudaFuncAttributeMaxDynamicSharedMemorySize, MsdSmem<WORDS>::kBytes));
+	CU(ctx, cudaOccupancyMaxActiveBlocksPerMultiprocessor(&ctx->occ_msd_part, msd_partition_kernel<WORDS>, MsdCfg<WORDS>::kThreads + 32, MsdSmem<WORDS>::kBytes));
+	CU(ctx, cudaFuncSetAttribute(msd_partition_kernel<WORDS, 1024>, cudaFuncAttributeMaxDynamicSharedMemorySize, MsdSmem<WORDS, 1024>::kBytes));
+	CU(ctx, cudaOccupancyMaxActiveBlocksPerMultiprocessor(&ctx->occ_msd_part_wide, msd_partition_kernel<WORDS, 1024>, MsdCfg<WORDS>::kThreads + 32, MsdSmem<WORDS, 1024>::kBytes));
 	if (ctx->occ_msd_part_wide < 1) ctx->occ_msd_part_wide = 1;
 	const int local_smem = msd_local_cap<WORDS>() * 8 * WORDS + (MsdLocalCfg<WORDS>::kThreads / 32) * 1024;
-	CU(cudaFuncSetAttribute(msd_local_sort_kernel<WORDS>, cudaFuncAttributeMaxDynamicSharedMemorySize, local_smem));
-	CU(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&ctx->occ_msd_local, msd_local_sort_kernel<WORDS>, MsdLocalCfg<WORDS>::kThreads, local_smem));
+	CU(ctx, cudaFuncSetAttribute(msd_local_sort_kernel<WORDS>, cudaFuncAttributeMaxDynamicSharedMemorySize, local_smem));
+	CU(ctx, cudaOccupancyMaxActiveBlocksPerMultiprocessor(&ctx->occ_msd_local, msd_local_sort_kernel<WORDS>, MsdLocalCfg<WORDS>::kThreads, local_smem));
 	if (ctx->occ_radix < 1) ctx->occ_radix = 1;
 	if (ctx->occ_expand < 1) ctx->occ_expand = 1;
 	if (ctx->occ_msd_part < 1) ctx->occ_msd_part = 1;
@@ -280,7 +246,7 @@ int launch_expand(kmcb200_ctx* ctx, const ExpandArgs& a, cudaStream_t st)
 	default: expand_kernel<WORDS, kExpandFilter><<<grid, ExpandCfg<WORDS>::kThreads, 0, st>>>(a); break;
 	}
 	ctx->launches++;
-	CU(cudaGetLastError());
+	CU(ctx, cudaGetLastError());
 	return 0;
 }
 
@@ -323,12 +289,12 @@ int ensure_msd(kmcb200_ctx* ctx, Slot& s, uint64_t n, uint32_t n_packs, uint32_t
 	const size_t items1 = std::max(msd_max_items1(n, n_packs), (size_t)(n / msd_tile<WORDS>()) + 2);
 	const size_t items2 = (size_t)(n / msd_tile<WORDS>()) + 260;
 	const size_t cells = std::max(256 * items1, (size_t)std::max(nd2, 256u) * items2);
-	if (int rc = ensure(ctx, s.msd_item_lo1, s.msd_item_lo1_cap, items1)) return rc;
-	if (int rc = ensure(ctx, s.msd_item_cnt1, s.msd_item_cnt1_cap, items1)) return rc;
-	if (int rc = ensure(ctx, s.msd_item_seg2, s.msd_item_seg2_cap, std::max(items1, items2))) return rc;
-	if (int rc = ensure(ctx, s.msd_cells, s.msd_cells_cap, cells)) return rc;
-	if (int rc = ensure(ctx, s.msd_cell_scan, s.msd_cell_scan_cap, cells)) return rc;
-	if (int rc = ensure(ctx, s.msd_block_sums, s.msd_block_sums_cap, cells / kCellChunk + 2)) return rc;
+	if (int rc = grow(ctx, s.msd_item_lo1, items1, kSlotSlack)) return rc;
+	if (int rc = grow(ctx, s.msd_item_cnt1, items1, kSlotSlack)) return rc;
+	if (int rc = grow(ctx, s.msd_item_seg2, std::max(items1, items2), kSlotSlack)) return rc;
+	if (int rc = grow(ctx, s.msd_cells, cells, kSlotSlack)) return rc;
+	if (int rc = grow(ctx, s.msd_cell_scan, cells, kSlotSlack)) return rc;
+	if (int rc = grow(ctx, s.msd_block_sums, cells / kCellChunk + 2, kSlotSlack)) return rc;
 	return 0;
 }
 
@@ -339,7 +305,7 @@ int launch_cell_scan(kmcb200_ctx* ctx, Slot& s, const uint32_t* n_items, uint32_
 	cell_scan_sums_kernel<<<1, 1024, 0, st>>>(s.msd_block_sums, n_items, nd, flags);
 	cell_scan_kernel<<<nb, 256, 0, st>>>(s.msd_cells, n_items, nd, s.msd_block_sums, s.msd_cell_scan, flags);
 	ctx->launches += 3;
-	CU(cudaGetLastError());
+	CU(ctx, cudaGetLastError());
 	return 0;
 }
 
@@ -359,7 +325,7 @@ int launch_lsd_sort(kmcb200_ctx* ctx, Slot& s, void* in, void* out, uint64_t n, 
 	a.reset_lut = reset_lut; a.reset_lut_entries = ctx->lut_entries; a.reset_result = reset_result;
 	const uint32_t grid = std::max(1u, std::min<uint32_t>(a.n_tiles, (uint32_t)(ctx->sm_count * ctx->occ_radix)));
 	void* params[] = {&a};
-	CU(cudaLaunchCooperativeKernel(reinterpret_cast<const void*>(lsd_sort_kernel<WORDS>), dim3(grid), dim3(SortCfg<WORDS>::kThreads), params, SortSmem<WORDS>::kBytes, st));
+	CU(ctx, cudaLaunchCooperativeKernel(reinterpret_cast<const void*>(lsd_sort_kernel<WORDS>), dim3(grid), dim3(SortCfg<WORDS>::kThreads), params, SortSmem<WORDS>::kBytes, st));
 	ctx->launches++;
 	return 0;
 }
@@ -391,13 +357,13 @@ int launch_sort(kmcb200_ctx* ctx, Slot& s, void* a, void* b, uint64_t n, uint32_
 	const bool msd = msd_path(ctx, n, key_bits);
 	if (hist_mode == kHistTotals && !msd) return fail(ctx, KMCB200_ERR_INVALID, "the records of this bin were not expanded");
 	const uint32_t top_shift = key_bits - 8;
-	if (int rc = ensure(ctx, s.desc, s.desc_cap, (size_t)n_tiles * 256, true)) return rc;
+	if (int rc = grow(ctx, s.desc, (size_t)n_tiles * 256, kSlotSlack, true)) return rc;
 	if (msd) if (int rc = ensure_msd<WORDS>(ctx, s, n, n_packs, choose_nd2<WORDS>(ctx, n, plan != nullptr))) return rc;      // (sized alike by stage_expand: no reallocation here when its cells are in use)
 
 	const bool hist_ready = hist_mode == kHistTiles || hist_mode == kHistTotals;
 	if (hist_mode == kHistNone) if (int rc = zero_async(ctx, s.zero, sizeof(ZeroBlock), st)) return rc;
 	int iv = 0;      // timed interval index
-	CU(cudaEventRecord(s.ev_pass[0], st));
+	CU(ctx, cudaEventRecord(s.ev_pass[0], st));
 	void* lsd_in = a; void* lsd_out = b;
 	const uint32_t* lsd_flag = nullptr;
 	if (msd) {
@@ -429,7 +395,7 @@ int launch_sort(kmcb200_ctx* ctx, Slot& s, void* a, void* b, uint64_t n, uint32_
 		}
 		if (hist_mode != kHistTotals) {
 			if (int rc = launch_cell_scan(ctx, s, items1.n_items, 256, max_items1, never, st)) return rc;
-			s.pass_names[iv] = "msd_scan_L1"; CU(cudaEventRecord(s.ev_pass[++iv], st));
+			s.pass_names[iv] = "msd_scan_L1"; CU(ctx, cudaEventRecord(s.ev_pass[++iv], st));
 		}
 		MsdBoundsArgs b1{};
 		b1.cell_scan = s.msd_cell_scan; b1.items = items1; b1.S = 1; b1.nd = 256; b1.n = n; b1.start = s.msd_start2;
@@ -444,7 +410,7 @@ int launch_sort(kmcb200_ctx* ctx, Slot& s, void* a, void* b, uint64_t n, uint32_
 			ea.mode = kExpandPartition; ea.recs = b; ea.l1_cursor = s.zero->l1_cursor; ea.l1_start = s.msd_start2;
 			if (int rc = launch_expand<WORDS>(ctx, ea, st)) return rc;
 			s.pass_names[iv] = "expand_scatter_L1";
-			CU(cudaEventRecord(s.ev_pass[++iv], st));
+			CU(ctx, cudaEventRecord(s.ev_pass[++iv], st));
 		} else {
 			MsdPartArgs p1{};
 			p1.in = a; p1.out = b; p1.items = items1; p1.cell_scan = s.msd_cell_scan; p1.shift = top_shift; p1.nd = 256;
@@ -452,7 +418,7 @@ int launch_sort(kmcb200_ctx* ctx, Slot& s, void* a, void* b, uint64_t n, uint32_
 			msd_partition_kernel<WORDS><<<pgrid1, MsdCfg<WORDS>::kThreads + 32, MsdSmem<WORDS>::kBytes, st>>>(p1);
 			ctx->launches++;
 			s.pass_names[iv] = "msd_partition_L1";
-			CU(cudaEventRecord(s.ev_pass[++iv], st));
+			CU(ctx, cudaEventRecord(s.ev_pass[++iv], st));
 			// (the item_seg table of the level-2 items shares its buffer with the all-zero level-1 table of kHistNone: partition first, bounds after)
 			msd_bounds_kernel<<<1, 1024, 0, st>>>(b1);
 			ctx->launches++;
@@ -470,14 +436,14 @@ int launch_sort(kmcb200_ctx* ctx, Slot& s, void* a, void* b, uint64_t n, uint32_
 			bb.cell_scan = s.msd_cell_scan; bb.items = items2; bb.S = 256; bb.nd = nd2; bb.n = n; bb.start = s.msd_start3; bb.cap = cap; bb.flags = flags; bb.tile = 0;
 			msd_bounds_flat_kernel<<<(256 * nd2 + 256) / 256 + 1, 256, 0, st>>>(bb);
 			ctx->launches++;
-			s.pass_names[iv] = "msd_count_L2"; CU(cudaEventRecord(s.ev_pass[++iv], st));
+			s.pass_names[iv] = "msd_count_L2"; CU(ctx, cudaEventRecord(s.ev_pass[++iv], st));
 			MsdPartArgs p2{};
 			p2.in = b; p2.out = a; p2.items = items2; p2.cell_scan = s.msd_cell_scan; p2.shift = top_shift - b2; p2.nd = nd2;
 			p2.flags = flags;
 			if (nd2 > 256) msd_partition_kernel<WORDS, 1024><<<pgrid2, MsdCfg<WORDS>::kThreads + 32, MsdSmem<WORDS, 1024>::kBytes, st>>>(p2);      // (a 512-digit instance with a third TMA buffer was slower)
 			else msd_partition_kernel<WORDS><<<pgrid2, MsdCfg<WORDS>::kThreads + 32, MsdSmem<WORDS>::kBytes, st>>>(p2);
 			ctx->launches++;
-			s.pass_names[iv] = "msd_partition_L2"; CU(cudaEventRecord(s.ev_pass[++iv], st));
+			s.pass_names[iv] = "msd_partition_L2"; CU(ctx, cudaEventRecord(s.ev_pass[++iv], st));
 		}
 		if (plan) {          // the caller counts the leaves (no sort of the duplicates)
 			plan->active = true;
@@ -489,7 +455,7 @@ int launch_sort(kmcb200_ctx* ctx, Slot& s, void* a, void* b, uint64_t n, uint32_
 			const uint32_t lgrid = (uint32_t)std::min<size_t>(lo.n_buckets, (size_t)ctx->sm_count * ctx->occ_msd_local);
 			msd_local_sort_kernel<WORDS><<<lgrid, MsdLocalCfg<WORDS>::kThreads, local_smem, st>>>(lo);
 			ctx->launches++;
-			s.pass_names[iv] = "msd_local_sort"; CU(cudaEventRecord(s.ev_pass[++iv], st));
+			s.pass_names[iv] = "msd_local_sort"; CU(ctx, cudaEventRecord(s.ev_pass[++iv], st));
 		}
 		lsd_in = b; lsd_out = a; lsd_flag = flags;
 		*result_in_b = final_in_b;
@@ -497,15 +463,15 @@ int launch_sort(kmcb200_ctx* ctx, Slot& s, void* a, void* b, uint64_t n, uint32_
 		*result_in_b = (key_bytes % 2) == 1;
 
 	if (plan && plan->active) {        // the caller runs the leaves first, then calls launch_lsd_fallback
-		CU(cudaGetLastError());
+		CU(ctx, cudaGetLastError());
 		s.n_passes_run = iv;
 		return 0;
 	}
 	// 8-bit LSD passes (one cooperative launch): the whole sort when the hybrid path is off (unless the bin is malformed: flags[1]),
 	// otherwise its fallback (returns at once unless flagged)
 	if (int rc = launch_lsd_sort<WORDS>(ctx, s, lsd_in, lsd_out, n, key_bytes, msd ? lsd_flag : &s.zero->msd_flags[1], msd ? kMsdFlagFallback : 0u, nullptr, nullptr, st)) return rc;
-	s.pass_names[iv] = msd ? "lsd_fallback(all passes)" : "lsd_sort(all passes)"; CU(cudaEventRecord(s.ev_pass[++iv], st));
-	CU(cudaGetLastError());
+	s.pass_names[iv] = msd ? "lsd_fallback(all passes)" : "lsd_sort(all passes)"; CU(ctx, cudaEventRecord(s.ev_pass[++iv], st));
+	CU(ctx, cudaGetLastError());
 	s.n_passes_run = iv;
 	return 0;
 }
@@ -516,7 +482,7 @@ int launch_count(kmcb200_ctx* ctx, Slot& s, const void* sorted, uint64_t n, uint
 {
 	constexpr int TILE = count_tile<WORDS>();
 	const uint32_t n_tiles = (uint32_t)((n + TILE - 1) / TILE);
-	if (int rc = ensure(ctx, s.cdesc, s.cdesc_cap, (size_t)n_tiles, true)) return rc;
+	if (int rc = grow(ctx, s.cdesc, (size_t)n_tiles, kSlotSlack, true)) return rc;
 	CountArgs a;
 	a.recs = sorted; a.n = n; a.n_tiles = n_tiles; a.k = ctx->prm.kmer_len; a.lut_prefix_len = ctx->prm.lut_prefix_len;
 	a.cutoff_min = ctx->prm.cutoff_min; a.cutoff_max = ctx->prm.cutoff_max; a.counter_max = ctx->prm.counter_max;
@@ -528,7 +494,7 @@ int launch_count(kmcb200_ctx* ctx, Slot& s, const void* sorted, uint64_t n, uint
 	const size_t smem = count_smem_bytes<WORDS>(ctx->suffix_bytes + ctx->counter_bytes);
 	count_emit_kernel<WORDS><<<std::min<uint32_t>(n_tiles, (uint32_t)ctx->sm_count * 6), CountCfg<WORDS>::kThreads, smem, st>>>(a);
 	ctx->launches++;
-	CU(cudaGetLastError());
+	CU(ctx, cudaGetLastError());
 	return 0;
 }
 
@@ -537,7 +503,7 @@ int launch_count(kmcb200_ctx* ctx, Slot& s, const void* sorted, uint64_t n, uint
 	 : (ctx)->words == 3 ? fn<3>(__VA_ARGS__) : fn<4>(__VA_ARGS__))
 
 // --------------------------------------------------------------------------------------------- stages
-int set_device(kmcb200_ctx* ctx) { CU(cudaSetDevice(ctx->prm.device)); return 0; }
+int set_device(kmcb200_ctx* ctx) { CU(ctx, cudaSetDevice(ctx->prm.device)); return 0; }
 
 int check_slot(kmcb200_ctx* ctx, uint32_t slot)
 {
@@ -560,29 +526,20 @@ struct ExpandMode {            // oversized bins: count the top 12 bits / keep o
 int upload_packs(kmcb200_ctx* ctx, Slot& s, uint64_t size, const uint64_t* pack_bytes, uint32_t n_packs, cudaStream_t st)
 {
 	const uint32_t np = (n_packs && pack_bytes) ? n_packs : 1;
-	if (np + 1 > s.packs_cap) {
+	if (np + 1 > s.d_pack_start.cap) {
 		const size_t cap = np + np / 4 + 64;
-		CU(cudaDeviceSynchronize());
-		for (int i = 0; i < kStageRing; ++i) {
-			if (s.h_pack_start[i]) CU(cudaFreeHost(s.h_pack_start[i]));
-			s.h_pack_start[i] = nullptr;
-		}
-		for (void* p : {(void*)s.d_pack_start, (void*)s.pack_nsk, (void*)s.pack_nk, (void*)s.pack_tbase, (void*)s.pack_kbase})
-			if (p) CU(cudaFree(p));
-		s.packs_cap = 0;
-		for (int i = 0; i < kStageRing; ++i) CU(cudaHostAlloc(reinterpret_cast<void**>(&s.h_pack_start[i]), cap * 8, cudaHostAllocDefault));
-		CU(cudaMalloc(reinterpret_cast<void**>(&s.d_pack_start), cap * 8));
-		CU(cudaMalloc(reinterpret_cast<void**>(&s.pack_nsk), cap * 4));
-		CU(cudaMalloc(reinterpret_cast<void**>(&s.pack_nk), cap * 4));
-		CU(cudaMalloc(reinterpret_cast<void**>(&s.pack_tbase), cap * 4));
-		CU(cudaMalloc(reinterpret_cast<void**>(&s.pack_kbase), cap * 8));
-		if (s.pack_done) CU(cudaFree(s.pack_done));
-		CU(cudaMalloc(reinterpret_cast<void**>(&s.pack_done), cap * 4));
-		s.packs_cap = cap;
+		CU(ctx, cudaDeviceSynchronize());
+		for (auto& h : s.h_pack_start) CU(ctx, h.alloc(cap));
+		CU(ctx, s.pack_nsk.alloc(cap));
+		CU(ctx, s.pack_nk.alloc(cap));
+		CU(ctx, s.pack_tbase.alloc(cap));
+		CU(ctx, s.pack_kbase.alloc(cap));
+		CU(ctx, s.pack_done.alloc(cap));
+		CU(ctx, s.d_pack_start.alloc(cap));
 	}
 	// (ring: the copy of an earlier bin may still be queued)
 	s.ring = (s.ring + 1) % kStageRing;
-	CU(cudaEventSynchronize(s.ev_pack[s.ring]));
+	CU(ctx, cudaEventSynchronize(s.ev_pack[s.ring]));
 	uint64_t* hps = s.h_pack_start[s.ring];
 	uint64_t acc = 0;
 	if (n_packs && pack_bytes) {
@@ -592,8 +549,8 @@ int upload_packs(kmcb200_ctx* ctx, Slot& s, uint64_t size, const uint64_t* pack_
 	hps[0] = 0;
 	hps[np] = acc;
 	if (acc != size) return fail(ctx, KMCB200_ERR_BIN_FORMAT, "expander packs cover %llu bytes but the bin has %llu", (unsigned long long)acc, (unsigned long long)size);
-	CU(cudaMemcpyAsync(s.d_pack_start, hps, (np + 1) * 8, cudaMemcpyHostToDevice, st));
-	CU(cudaEventRecord(s.ev_pack[s.ring], st));
+	CU(ctx, cudaMemcpyAsync(s.d_pack_start, hps, (np + 1) * 8, cudaMemcpyHostToDevice, st));
+	CU(ctx, cudaEventRecord(s.ev_pack[s.ring], st));
 	return 0;
 }
 
@@ -618,12 +575,12 @@ int stage_expand(kmcb200_ctx* ctx, Slot& s, const uint8_t* d_bin, uint64_t size,
 	const bool msd_items = mode == kExpandAll || mode == kExpandPartition;          // level 1 of the sort follows: its buffers are sized here
 	s.hist_mode = mode == kExpandAll ? kHistTiles : mode == kExpandPartition ? kHistTotals : kHistNone;
 
-	if (int rc = ensure(ctx, s.sk_off, s.sk_off_cap, size / min_rec + 2)) return rc;
-	if (int rc = ensure(ctx, s.sk_kpre, s.sk_kpre_cap, size / min_rec + 2)) return rc;
-	if (int rc = ensure(ctx, s.tile_first, s.tile_first_cap, size * 4 / kExpandMinTile + np + 2)) return rc;
+	if (int rc = grow(ctx, s.sk_off, size / min_rec + 2, kSlotSlack)) return rc;
+	if (int rc = grow(ctx, s.sk_kpre, size / min_rec + 2, kSlotSlack)) return rc;
+	if (int rc = grow(ctx, s.tile_first, size * 4 / kExpandMinTile + np + 2, kSlotSlack)) return rc;
 	const uint64_t n_bound = n_rec == kExpandUnknownRecs ? size * 4 : n_rec;        // a record of 1 + ceil((k+a)/4) bytes holds a+1 k-mers: < 4 per byte
-	if (int rc = ensure(ctx, s.tile_pack, s.tile_pack_cap, n_bound / kExpandMinTile + np + 2)) return rc;
-	if (int rc = ensure(ctx, s.tile_desc, s.tile_desc_cap, 2 * (n_bound / kExpandMinTile + np + 2))) return rc;
+	if (int rc = grow(ctx, s.tile_pack, n_bound / kExpandMinTile + np + 2, kSlotSlack)) return rc;
+	if (int rc = grow(ctx, s.tile_desc, 2 * (n_bound / kExpandMinTile + np + 2), kSlotSlack)) return rc;
 
 	ExpandArgs a;
 	a.bin = d_bin; a.size = size; a.pack_start = s.d_pack_start; a.n_packs = np; a.k = k; a.min_rec_bytes = min_rec;
@@ -645,7 +602,7 @@ int stage_expand(kmcb200_ctx* ctx, Slot& s, const uint8_t* d_bin, uint64_t size,
 	a.l1_cursor = nullptr; a.l1_start = nullptr;
 	if (mode == kExpandPartition) s.expand_args = a;
 
-	bin_init_kernel<<<64, 256, 0, st>>>(reinterpret_cast<uint32_t*>(s.zero), (uint32_t)(sizeof(ZeroBlock) / 4), reinterpret_cast<uint32_t*>(zero_lut),
+	bin_init_kernel<<<64, 256, 0, st>>>(reinterpret_cast<uint32_t*>(s.zero.get()), (uint32_t)(sizeof(ZeroBlock) / 4), reinterpret_cast<uint32_t*>(zero_lut),
 		(size_t)ctx->lut_entries * 2, reinterpret_cast<uint32_t*>(zero_result));
 	if (s.have_extras && msd_items) {          // N4: stage 1 handed over the length bytes: two prefix sums per pack instead of the walk
 		index_from_extras_kernel<<<np, 1024, 0, st>>>(a, s.d_extras, s.d_pack_rec);
@@ -663,10 +620,10 @@ int stage_expand(kmcb200_ctx* ctx, Slot& s, const uint8_t* d_bin, uint64_t size,
 	scan_packs_kernel<<<1, 1024, 0, st>>>(a);
 	tile_desc_kernel<<<(uint32_t)((a.tile_pack_cap + 255) / 256), 256, 0, st>>>(a);
 	ctx->launches += 2;
-	CU(cudaGetLastError());
+	CU(ctx, cudaGetLastError());
 	if (st_expand != st) {
-		CU(cudaEventRecord(s.ev_walk, st));
-		CU(cudaStreamWaitEvent(st_expand, s.ev_walk, 0));
+		CU(ctx, cudaEventRecord(s.ev_walk, st));
+		CU(ctx, cudaStreamWaitEvent(st_expand, s.ev_walk, 0));
 	}
 	if (mode == kExpandPartition) return 0;          // the bin is expanded by level 1 of the sort, once its buckets are known
 	return DISPATCH_WORDS(ctx, launch_expand, ctx, a, st_expand);
@@ -680,7 +637,7 @@ int stage_count(kmcb200_ctx* ctx, Slot& s, const void* sorted, uint64_t n, uint8
 	if (!outputs_zeroed) {
 		bin_init_kernel<<<64, 256, 0, st>>>(&s.zero->counters[kMaxPasses], 1u, reinterpret_cast<uint32_t*>(d_lut), (size_t)ctx->lut_entries * 2, reinterpret_cast<uint32_t*>(d_result));
 		ctx->launches++;
-		CU(cudaGetLastError());
+		CU(ctx, cudaGetLastError());
 	}
 	if (n == 0) return 0;
 	return DISPATCH_WORDS(ctx, launch_count, ctx, s, sorted, n, d_out, out_capacity, d_lut, d_result, guarded ? &s.zero->msd_flags[1] : nullptr, 0u, st, out_base);
@@ -718,12 +675,12 @@ int setup_leaf_cta(kmcb200_ctx* ctx)
 {
 	const int smem = (int)sizeof(LcSmem<NWARPS, SLOT_BITS>);
 	int occ_t = 1, occ_f = 1;
-	CU((cudaFuncSetAttribute(leaf_hash_cta_kernel<NWARPS, SLOT_BITS, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem)));
-	CU((cudaFuncSetAttribute(leaf_hash_cta_kernel<NWARPS, SLOT_BITS, true>, cudaFuncAttributePreferredSharedMemoryCarveout, 100)));
-	CU((cudaFuncSetAttribute(leaf_hash_cta_kernel<NWARPS, SLOT_BITS, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem)));
-	CU((cudaFuncSetAttribute(leaf_hash_cta_kernel<NWARPS, SLOT_BITS, false>, cudaFuncAttributePreferredSharedMemoryCarveout, 100)));
-	CU((cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ_t, leaf_hash_cta_kernel<NWARPS, SLOT_BITS, true>, 32 * NWARPS, smem)));
-	CU((cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ_f, leaf_hash_cta_kernel<NWARPS, SLOT_BITS, false>, 32 * NWARPS, smem)));
+	CU(ctx, (cudaFuncSetAttribute(leaf_hash_cta_kernel<NWARPS, SLOT_BITS, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem)));
+	CU(ctx, (cudaFuncSetAttribute(leaf_hash_cta_kernel<NWARPS, SLOT_BITS, true>, cudaFuncAttributePreferredSharedMemoryCarveout, 100)));
+	CU(ctx, (cudaFuncSetAttribute(leaf_hash_cta_kernel<NWARPS, SLOT_BITS, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem)));
+	CU(ctx, (cudaFuncSetAttribute(leaf_hash_cta_kernel<NWARPS, SLOT_BITS, false>, cudaFuncAttributePreferredSharedMemoryCarveout, 100)));
+	CU(ctx, (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ_t, leaf_hash_cta_kernel<NWARPS, SLOT_BITS, true>, 32 * NWARPS, smem)));
+	CU(ctx, (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ_f, leaf_hash_cta_kernel<NWARPS, SLOT_BITS, false>, 32 * NWARPS, smem)));
 	ctx->occ_leaf_cta = std::max(1, std::min(occ_t, occ_f));
 	return 0;
 }
@@ -755,7 +712,7 @@ int launch_leaves(kmcb200_ctx* ctx, const LeafArgs& la, uint64_t n_rec, cudaStre
 		else leaf_hash_wide_kernel<WORDS, kLeafSlotBits, false><<<hgrid, 32 * kLwWarps, hsmem, st>>>(la);
 	}
 	ctx->launches++;
-	CU(cudaGetLastError());
+	CU(ctx, cudaGetLastError());
 	return 0;
 }
 
@@ -765,7 +722,7 @@ int launch_heavy_leaves(kmcb200_ctx* ctx, const LeafArgs& la, cudaStream_t st)
 	const size_t smem = sizeof(LwSmem<kLeafSlotBits>) * kLwWarps;
 	leaf_warp_kernel<kLeafSlotBits><<<(uint32_t)ctx->sm_count, 32 * kLwWarps, smem, st>>>(la);
 	ctx->launches++;
-	CU(cudaGetLastError());
+	CU(ctx, cudaGetLastError());
 	return 0;
 }
 
@@ -775,22 +732,22 @@ int setup_leaves(kmcb200_ctx* ctx)
 	const int hsmem = (int)(sizeof(LhSmem<kLeafSlotBits>) * kLwWarps);
 	int occ_t = 1, occ_f = 1;
 	if constexpr (WORDS == 1) {
-		CU((cudaFuncSetAttribute(leaf_warp_kernel<kLeafSlotBits>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(sizeof(LwSmem<kLeafSlotBits>) * kLwWarps))));
-		CU((cudaFuncSetAttribute(leaf_hash_kernel<kLeafSlotBits, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, hsmem)));
-		CU((cudaFuncSetAttribute(leaf_hash_kernel<kLeafSlotBits, true>, cudaFuncAttributePreferredSharedMemoryCarveout, 100)));
-		CU((cudaFuncSetAttribute(leaf_hash_kernel<kLeafSlotBits, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, hsmem)));
-		CU((cudaFuncSetAttribute(leaf_hash_kernel<kLeafSlotBits, false>, cudaFuncAttributePreferredSharedMemoryCarveout, 100)));
-		CU((cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ_t, leaf_hash_kernel<kLeafSlotBits, true>, 32 * kLwWarps, hsmem)));
-		CU((cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ_f, leaf_hash_kernel<kLeafSlotBits, false>, 32 * kLwWarps, hsmem)));
+		CU(ctx, (cudaFuncSetAttribute(leaf_warp_kernel<kLeafSlotBits>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(sizeof(LwSmem<kLeafSlotBits>) * kLwWarps))));
+		CU(ctx, (cudaFuncSetAttribute(leaf_hash_kernel<kLeafSlotBits, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, hsmem)));
+		CU(ctx, (cudaFuncSetAttribute(leaf_hash_kernel<kLeafSlotBits, true>, cudaFuncAttributePreferredSharedMemoryCarveout, 100)));
+		CU(ctx, (cudaFuncSetAttribute(leaf_hash_kernel<kLeafSlotBits, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, hsmem)));
+		CU(ctx, (cudaFuncSetAttribute(leaf_hash_kernel<kLeafSlotBits, false>, cudaFuncAttributePreferredSharedMemoryCarveout, 100)));
+		CU(ctx, (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ_t, leaf_hash_kernel<kLeafSlotBits, true>, 32 * kLwWarps, hsmem)));
+		CU(ctx, (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ_f, leaf_hash_kernel<kLeafSlotBits, false>, 32 * kLwWarps, hsmem)));
 		if (ctx->leaf_cta)
 			if (int rc = DISPATCH_CTA(ctx, setup_leaf_cta, ctx)) return rc;
 	} else {
-		CU((cudaFuncSetAttribute(leaf_hash_wide_kernel<WORDS, kLeafSlotBits, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, hsmem)));
-		CU((cudaFuncSetAttribute(leaf_hash_wide_kernel<WORDS, kLeafSlotBits, true>, cudaFuncAttributePreferredSharedMemoryCarveout, 100)));
-		CU((cudaFuncSetAttribute(leaf_hash_wide_kernel<WORDS, kLeafSlotBits, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, hsmem)));
-		CU((cudaFuncSetAttribute(leaf_hash_wide_kernel<WORDS, kLeafSlotBits, false>, cudaFuncAttributePreferredSharedMemoryCarveout, 100)));
-		CU((cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ_t, leaf_hash_wide_kernel<WORDS, kLeafSlotBits, true>, 32 * kLwWarps, hsmem)));
-		CU((cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ_f, leaf_hash_wide_kernel<WORDS, kLeafSlotBits, false>, 32 * kLwWarps, hsmem)));
+		CU(ctx, (cudaFuncSetAttribute(leaf_hash_wide_kernel<WORDS, kLeafSlotBits, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, hsmem)));
+		CU(ctx, (cudaFuncSetAttribute(leaf_hash_wide_kernel<WORDS, kLeafSlotBits, true>, cudaFuncAttributePreferredSharedMemoryCarveout, 100)));
+		CU(ctx, (cudaFuncSetAttribute(leaf_hash_wide_kernel<WORDS, kLeafSlotBits, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, hsmem)));
+		CU(ctx, (cudaFuncSetAttribute(leaf_hash_wide_kernel<WORDS, kLeafSlotBits, false>, cudaFuncAttributePreferredSharedMemoryCarveout, 100)));
+		CU(ctx, (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ_t, leaf_hash_wide_kernel<WORDS, kLeafSlotBits, true>, 32 * kLwWarps, hsmem)));
+		CU(ctx, (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ_f, leaf_hash_wide_kernel<WORDS, kLeafSlotBits, false>, 32 * kLwWarps, hsmem)));
 	}
 	ctx->occ_leaf_hash = std::max(1, std::min(occ_t, occ_f));
 	return 0;
@@ -811,14 +768,14 @@ int run_sort_count_leaves(kmcb200_ctx* ctx, Slot& s, uint64_t n_rec, uint32_t np
 	LeafPlan plan;
 	if (int rc = launch_sort<WORDS>(ctx, s, ra, rb, n_rec, ctx->key_bytes, 2u * ctx->prm.kmer_len - block_bits, from_blocks ? (int)kHistNone : s.hist_mode, np_eff, st, &in_b, &plan)) return rc;
 	if (!plan.active) {          // small bin: plain LSD passes, classic count
-		CU(cudaEventRecord(s.ev_sort, st));
+		CU(ctx, cudaEventRecord(s.ev_sort, st));
 		s.ran_sort = true;
 		const void* sorted = in_b ? rb : ra;
 		return stage_count(ctx, s, sorted, n_rec, d_out, out_capacity, d_lut, d_result, st, outputs_zeroed, true, out_base);
 	}
 	const uint32_t ob = ctx->suffix_bytes + ctx->counter_bytes;
 	const size_t pad = (size_t)((ob + 7) / 8) * 8;
-	if (int rc = ensure(ctx, s.leaf_tmp, s.leaf_tmp_cap, (size_t)n_rec * pad + 64)) return rc;
+	if (int rc = grow(ctx, s.leaf_tmp, (size_t)n_rec * pad + 64, kSlotSlack)) return rc;
 	if (!outputs_zeroed) {
 		bin_init_kernel<<<64, 256, 0, st>>>(nullptr, 0u, reinterpret_cast<uint32_t*>(d_lut), (size_t)ctx->lut_entries * 2, reinterpret_cast<uint32_t*>(d_result));
 		ctx->launches++;
@@ -840,13 +797,13 @@ int run_sort_count_leaves(kmcb200_ctx* ctx, Slot& s, uint64_t n_rec, uint32_t np
 	leaf_gather_kernel<<<(plan.n_leaves + 7) / 8, 256, 0, st>>>(s.leaf_tmp, plan.start, s.leaf_emit, s.leaf_off, plan.n_leaves, ob, d_out, d_result, flags, out_base);
 	ctx->launches += 2;
 	int iv = s.n_passes_run;
-	s.pass_names[iv] = "leaf_count"; CU(cudaEventRecord(s.ev_pass[++iv], st));
+	s.pass_names[iv] = "leaf_count"; CU(ctx, cudaEventRecord(s.ev_pass[++iv], st));
 	// fallback (two launches that return at once unless a leaf could not be counted): all LSD passes from the level-1 output in one
 	// cooperative kernel (which first forgets what the leaves added to the LUT / statistics), then the classic count
 	if (int rc = launch_lsd_sort<WORDS>(ctx, s, rb, ra, n_rec, ctx->key_bytes, flags, kMsdFlagFallback, d_lut, d_result, st)) return rc;
-	s.pass_names[iv] = "lsd_fallback(all passes)"; CU(cudaEventRecord(s.ev_pass[++iv], st));
+	s.pass_names[iv] = "lsd_fallback(all passes)"; CU(ctx, cudaEventRecord(s.ev_pass[++iv], st));
 	s.n_passes_run = iv;
-	CU(cudaEventRecord(s.ev_sort, st));
+	CU(ctx, cudaEventRecord(s.ev_sort, st));
 	s.ran_sort = true;
 	const void* sorted = (ctx->key_bytes % 2 == 0) ? rb : ra;
 	return launch_count<WORDS>(ctx, s, sorted, n_rec, d_out, out_capacity, d_lut, d_result, flags, kMsdFlagFallback, st, out_base);
@@ -859,29 +816,29 @@ int run_bin(kmcb200_ctx* ctx, Slot& s, const uint8_t* d_bin, uint64_t size, uint
 {
 	const size_t rec_bytes = (size_t)ctx->words * 8;
 	s.ran_expand = s.ran_sort = s.ran_count = false;
-	CU(cudaEventRecord(s.ev_begin, st));
+	CU(ctx, cudaEventRecord(s.ev_begin, st));
 	if (n_rec == 0 || size == 0) {
 		if (n_rec != 0 || size != 0) return fail(ctx, KMCB200_ERR_BIN_FORMAT, "bin with size=%llu but n_rec=%llu", (unsigned long long)size, (unsigned long long)n_rec);
 		if (int rc = stage_count(ctx, s, nullptr, 0, d_out, out_capacity, d_lut, d_result, st)) return rc;
 		if (host_result) { finish_result_kernel<<<1, 32, 0, st>>>(d_result, 0, nullptr, nullptr, host_result); ctx->launches++; }
-		CU(cudaEventRecord(s.ev_expand, st)); CU(cudaEventRecord(s.ev_sort, st)); CU(cudaEventRecord(s.ev_count, st));
+		CU(ctx, cudaEventRecord(s.ev_expand, st)); CU(ctx, cudaEventRecord(s.ev_sort, st)); CU(ctx, cudaEventRecord(s.ev_count, st));
 		s.n_passes_run = 0;
 		return 0;
 	}
-	if (int rc = ensure(ctx, s.recs_a, s.recs_a_cap, n_rec * rec_bytes)) return rc;
-	if (int rc = ensure(ctx, s.recs_b, s.recs_b_cap, n_rec * rec_bytes)) return rc;
+	if (int rc = grow(ctx, s.recs_a, n_rec * rec_bytes, kSlotSlack)) return rc;
+	if (int rc = grow(ctx, s.recs_b, n_rec * rec_bytes, kSlotSlack)) return rc;
 	// a bin of one-word records that takes the MSD path is expanded once, straight into its level-1 buckets, whose sizes the pack walk
 	// counts (expand.cuh, kExpandPartition): its records are never written in tile order and read back by a separate partition pass
 	ExpandMode em;
 	if (expand_partition_supported<1>() && ctx->words == 1 && n_rec < (1ull << 32) && msd_path(ctx, n_rec, 2u * ctx->prm.kmer_len)) em.mode = kExpandPartition;
 	if (int rc = stage_expand(ctx, s, d_bin, size, n_rec, pack_bytes, n_packs, s.recs_a, st, em, packs_uploaded, d_lut, d_result, st_walk)) return rc;
-	CU(cudaEventRecord(s.ev_expand, st));
+	CU(ctx, cudaEventRecord(s.ev_expand, st));
 	s.ran_expand = true;
 	const uint32_t np_eff = (n_packs && pack_bytes) ? n_packs : 1u;
 	if (int rc = DISPATCH_WORDS(ctx, run_sort_count_leaves, ctx, s, n_rec, np_eff, d_out, out_capacity, d_lut, d_result, st, false, 0u, 0u, true)) return rc;
 	finish_result_kernel<<<1, 32, 0, st>>>(d_result, n_rec, s.zero->status, s.zero->msd_flags, host_result);
 	ctx->launches++;
-	CU(cudaEventRecord(s.ev_count, st));
+	CU(ctx, cudaEventRecord(s.ev_count, st));
 	s.ran_count = true;
 	return 0;
 }
@@ -932,20 +889,20 @@ int plan_chunks(kmcb200_ctx* ctx, uint64_t size, const uint64_t* pack_bytes, uin
 int count_top12(kmcb200_ctx* ctx, Slot& s, const std::vector<BinChunk>& chunks, const uint64_t* pack_bytes, std::vector<uint64_t>& hist, cudaStream_t st)
 {
 	const uint32_t k = ctx->prm.kmer_len;
-	if (!s.d_hist12) { CU(cudaMalloc(reinterpret_cast<void**>(&s.d_hist12), 4096 * 8)); }
+	if (!s.d_hist12) CU(ctx, s.d_hist12.alloc(4096));
 	if (int rc = zero_async(ctx, s.d_hist12, 4096 * 8, st)) return rc;
 	ExpandMode em;
 	em.mode = kExpandCount12; em.fshift = 2 * k - 12; em.hist12 = s.d_hist12;
 	for (const BinChunk& c : chunks) {
 		if (int rc = stage_expand(ctx, s, s.d_bin + c.dev_off, c.bytes, kExpandUnknownRecs, pack_bytes + c.pack0, c.npacks, nullptr, st, em)) return rc;
 		uint32_t status = 0;
-		CU(cudaMemcpyAsync(&status, s.zero->status, 4, cudaMemcpyDeviceToHost, st));
-		CU(cudaStreamSynchronize(st));
+		CU(ctx, cudaMemcpyAsync(&status, s.zero->status, 4, cudaMemcpyDeviceToHost, st));
+		CU(ctx, cudaStreamSynchronize(st));
 		if (status & kErrPackWalk) return fail(ctx, KMCB200_ERR_BIN_FORMAT, "bin format error: an expander pack does not end on a record boundary");
 	}
 	hist.assign(4096, 0);
-	CU(cudaMemcpyAsync(hist.data(), s.d_hist12, 4096 * 8, cudaMemcpyDeviceToHost, st));
-	CU(cudaStreamSynchronize(st));
+	CU(ctx, cudaMemcpyAsync(hist.data(), s.d_hist12, 4096 * 8, cudaMemcpyDeviceToHost, st));
+	CU(ctx, cudaStreamSynchronize(st));
 	return 0;
 }
 
@@ -984,34 +941,24 @@ int sort_count_block(kmcb200_ctx* ctx, Slot& s, void* region, void* rb, const Ke
 	if (int rc = DISPATCH_WORDS(ctx, run_sort_count_leaves, ctx, s, b.n, 1u, d_out, out_capacity, s.d_lut, s.d_result, st, true, b.bits, b.prefix, false, tot_res + 4, region, rb)) return rc;
 	accumulate_block_kernel<<<64, 256, 0, st>>>(tot_lut, s.d_lut, ctx->lut_entries, tot_res, s.d_result, appended, b.n);
 	ctx->launches++;
-	CU(cudaGetLastError());
+	CU(ctx, cudaGetLastError());
 	return 0;
 }
 
 // uploads the tables of a scattering expansion (block of every 12-bit prefix, first record of every block's region) and zeroes the counters
 int setup_scatter(kmcb200_ctx* ctx, Slot& s, const std::vector<KeyBlock>& blocks, const std::vector<uint64_t>& region_start, cudaStream_t st)
 {
-	if (!s.d_out_counter || s.out_counter_cap < blocks.size() + 1) {
-		if (s.d_out_counter) CU(cudaFree(s.d_out_counter));
-		s.d_out_counter = nullptr;
-		s.out_counter_cap = std::max<size_t>(blocks.size() + 1, 64);
-		CU(cudaMalloc(reinterpret_cast<void**>(&s.d_out_counter), s.out_counter_cap * 8));
-	}
+	if (int rc = grow(ctx, s.d_out_counter, blocks.size() + 1, kBlockTableSlack)) return rc;
 	std::vector<uint16_t> h_blk(4096, (uint16_t)0xFFFF);          // prefixes outside these blocks: skipped
 	for (size_t i = 0; i < blocks.size(); ++i) {
 		const uint32_t lo = blocks[i].prefix << (12 - blocks[i].bits), len = 1u << (12 - blocks[i].bits);
 		for (uint32_t q = lo; q < lo + len; ++q) h_blk[q] = (uint16_t)i;
 	}
-	if (!s.d_blk_of_prefix) CU(cudaMalloc(reinterpret_cast<void**>(&s.d_blk_of_prefix), 4096 * 2));
-	if (!s.d_region_start || s.region_cap < blocks.size()) {
-		if (s.d_region_start) CU(cudaFree(s.d_region_start));
-		s.d_region_start = nullptr;
-		s.region_cap = std::max<size_t>(blocks.size(), 64);
-		CU(cudaMalloc(reinterpret_cast<void**>(&s.d_region_start), s.region_cap * 8));
-	}
-	CU(cudaMemcpyAsync(s.d_blk_of_prefix, h_blk.data(), 4096 * 2, cudaMemcpyHostToDevice, st));
-	CU(cudaMemcpyAsync(s.d_region_start, region_start.data(), blocks.size() * 8, cudaMemcpyHostToDevice, st));
-	CU(cudaStreamSynchronize(st));          // (h_blk goes out of scope)
+	if (!s.d_blk_of_prefix) CU(ctx, s.d_blk_of_prefix.alloc(4096));
+	if (int rc = grow(ctx, s.d_region_start, blocks.size(), kBlockTableSlack)) return rc;
+	CU(ctx, cudaMemcpyAsync(s.d_blk_of_prefix, h_blk.data(), 4096 * 2, cudaMemcpyHostToDevice, st));
+	CU(ctx, cudaMemcpyAsync(s.d_region_start, region_start.data(), blocks.size() * 8, cudaMemcpyHostToDevice, st));
+	CU(ctx, cudaStreamSynchronize(st));          // (h_blk goes out of scope)
 	return zero_async(ctx, s.d_out_counter, blocks.size() * 8, st);
 }
 
@@ -1023,7 +970,7 @@ int scatter_chunks(kmcb200_ctx* ctx, Slot& s, const std::vector<BinChunk>& chunk
 	for (const BinChunk& c : chunks)
 		if (int rc = stage_expand(ctx, s, s.d_bin + c.dev_off, c.bytes, kExpandUnknownRecs, pack_bytes + c.pack0, c.npacks, dst, st, es)) return rc;
 	s.ran_expand = false;
-	CU(cudaEventRecord(s.ev_expand, st));
+	CU(ctx, cudaEventRecord(s.ev_expand, st));
 	return 0;
 }
 
@@ -1042,15 +989,14 @@ int run_key_blocks(kmcb200_ctx* ctx, Slot& s, const std::vector<BinChunk>& chunk
 	bool scatter = ctx->scatter_blocks && blocks.size() > 1 && blocks.size() <= kExpandMaxBlocks && 2 * k >= 24;
 	if (scatter) {          // does the bin-wide buffer fit next to what a block needs (scratch records, padded leaf output, tables)?
 		size_t free_b = 0, total_b = 0;
-		CU(cudaMemGetInfo(&free_b, &total_b));
-		const uint64_t have = (uint64_t)free_b + s.recs_a_cap + s.recs_b_cap + s.leaf_tmp_cap;          // (the slot's own buffers are re-sized below)
+		CU(ctx, cudaMemGetInfo(&free_b, &total_b));
+		const uint64_t have = (uint64_t)free_b + s.recs_a.cap + s.recs_b.cap + s.leaf_tmp.cap;          // (the slot's own buffers are re-sized below)
 		const uint64_t need = sum_n * rec_bytes + max_n * (rec_bytes + 8 * ((ctx->suffix_bytes + ctx->counter_bytes + 7) / 8) + 4) + (256ull << 20);
 		scatter = need <= (uint64_t)(0.9 * (double)have);
 	}
-	s.last_scatter = scatter;
 	if (scatter) {
-		if (int rc = ensure(ctx, s.recs_a, s.recs_a_cap, (sum_n + blocks.size() + 2) * rec_bytes)) return rc;          // the bin-wide record buffer (+ the regions' alignment gaps)
-		if (int rc = ensure(ctx, s.recs_b, s.recs_b_cap, max_n * rec_bytes)) return rc;          // one block's scratch
+		if (int rc = grow(ctx, s.recs_a, (sum_n + blocks.size() + 2) * rec_bytes, kSlotSlack)) return rc;          // the bin-wide record buffer (+ the regions' alignment gaps)
+		if (int rc = grow(ctx, s.recs_b, max_n * rec_bytes, kSlotSlack)) return rc;          // one block's scratch
 		std::vector<uint64_t> h_reg(blocks.size());
 		uint64_t acc = 0;
 		for (size_t i = 0; i < blocks.size(); ++i) {
@@ -1063,9 +1009,9 @@ int run_key_blocks(kmcb200_ctx* ctx, Slot& s, const std::vector<BinChunk>& chunk
 			if (int rc = sort_count_block(ctx, s, s.recs_a + h_reg[i] * rec_bytes, s.recs_b, blocks[i], d_out, out_capacity, tot_lut, tot_res, s.d_out_counter + i, st)) return rc;
 		return 0;
 	}
-	if (!s.d_out_counter) { s.out_counter_cap = 64; CU(cudaMalloc(reinterpret_cast<void**>(&s.d_out_counter), s.out_counter_cap * 8)); }
-	if (int rc = ensure(ctx, s.recs_a, s.recs_a_cap, max_n * rec_bytes)) return rc;          // (sized once: no reallocation, no device synchronisation inside the loop)
-	if (int rc = ensure(ctx, s.recs_b, s.recs_b_cap, max_n * rec_bytes)) return rc;
+	if (int rc = grow(ctx, s.d_out_counter, 1, kBlockTableSlack)) return rc;
+	if (int rc = grow(ctx, s.recs_a, max_n * rec_bytes, kSlotSlack)) return rc;          // (sized once: no reallocation, no device synchronisation inside the loop)
+	if (int rc = grow(ctx, s.recs_b, max_n * rec_bytes, kSlotSlack)) return rc;
 	for (const KeyBlock& b : blocks) {
 		if (int rc = zero_async(ctx, s.d_out_counter, 8, st)) return rc;
 		ExpandMode ef;
@@ -1075,7 +1021,7 @@ int run_key_blocks(kmcb200_ctx* ctx, Slot& s, const std::vector<BinChunk>& chunk
 		for (const BinChunk& c : chunks)
 			if (int rc = stage_expand(ctx, s, s.d_bin + c.dev_off, c.bytes, kExpandUnknownRecs, pack_bytes + c.pack0, c.npacks, s.recs_a, st, ef)) return rc;
 		s.ran_expand = false;
-		CU(cudaEventRecord(s.ev_expand, st));
+		CU(ctx, cudaEventRecord(s.ev_expand, st));
 		if (int rc = sort_count_block(ctx, s, s.recs_a, s.recs_b, b, d_out, out_capacity, tot_lut, tot_res, s.d_out_counter, st)) return rc;
 	}
 	return 0;
@@ -1084,8 +1030,8 @@ int run_key_blocks(kmcb200_ctx* ctx, Slot& s, const std::vector<BinChunk>& chunk
 int ensure_totals(kmcb200_ctx* ctx, Slot& s, cudaStream_t st)
 {
 	if (!s.tot_lut) {
-		CU(cudaMalloc(reinterpret_cast<void**>(&s.tot_lut), ctx->lut_entries * 8));
-		CU(cudaMalloc(reinterpret_cast<void**>(&s.tot_res), 64));
+		CU(ctx, s.tot_res.alloc(8));
+		CU(ctx, s.tot_lut.alloc(ctx->lut_entries));
 	}
 	if (int rc = zero_async(ctx, s.tot_lut, ctx->lut_entries * 8, st)) return rc;
 	return zero_async(ctx, s.tot_res, 64, st);
@@ -1099,8 +1045,8 @@ int run_oversized_bin(kmcb200_ctx* ctx, Slot& s, const uint8_t* h_bin, uint64_t 
 	std::vector<BinChunk> chunks;
 	uint64_t dev_bytes = 0;
 	if (int rc = plan_chunks(ctx, size, pack_bytes, n_packs, chunks, &dev_bytes)) return rc;
-	if (int rc = ensure(ctx, s.d_bin, s.bin_cap, dev_bytes + 64)) return rc;
-	for (const BinChunk& c : chunks) CU(cudaMemcpyAsync(s.d_bin + c.dev_off, h_bin + c.byte0, c.bytes, cudaMemcpyHostToDevice, st));
+	if (int rc = grow(ctx, s.d_bin, dev_bytes + 64, kSlotSlack)) return rc;
+	for (const BinChunk& c : chunks) CU(ctx, cudaMemcpyAsync(s.d_bin + c.dev_off, h_bin + c.byte0, c.bytes, cudaMemcpyHostToDevice, st));
 	std::vector<KeyBlock> blocks;
 	if (n_rec <= ctx->max_block_records) blocks.push_back(KeyBlock{0, 0, n_rec});          // only too long: one block, the appended count checks n_rec
 	else {
@@ -1113,27 +1059,26 @@ int run_oversized_bin(kmcb200_ctx* ctx, Slot& s, const uint8_t* h_bin, uint64_t 
 		// key blocks of the preferred size (leaves of 1-2 K records: the leaf kernel's best case) when ONE scattering expansion can serve them
 		// all - i.e. the records fit in HBM once; otherwise as large as one sort can take, because then every block costs an expansion
 		size_t free_b = 0, total_b = 0;
-		CU(cudaMemGetInfo(&free_b, &total_b));
+		CU(ctx, cudaMemGetInfo(&free_b, &total_b));
 		const uint64_t rec_b = (uint64_t)ctx->words * 8;
-		const bool fits_once = ctx->scatter_blocks && (double)n_rec * rec_b + (double)ctx->key_block_records * (rec_b + 12) * 1.5 < 0.85 * (double)(free_b + s.recs_a_cap + s.recs_b_cap + s.leaf_tmp_cap);
+		const bool fits_once = ctx->scatter_blocks && (double)n_rec * rec_b + (double)ctx->key_block_records * (rec_b + 12) * 1.5 < 0.85 * (double)(free_b + s.recs_a.cap + s.recs_b.cap + s.leaf_tmp.cap);
 		const uint64_t limit = fits_once ? std::min(ctx->max_block_records, ctx->key_block_records) : ctx->max_block_records;
 		if (int rc = bisect_blocks(ctx, hist, 0, 4096, limit, blocks)) return rc;
 		if (blocks.size() > kExpandMaxBlocks) { blocks.clear(); if (int rc = bisect_blocks(ctx, hist, 0, 4096, ctx->max_block_records, blocks)) return rc; }
 	}
 	const uint32_t ob = ctx->suffix_bytes + ctx->counter_bytes;
-	if (int rc = ensure(ctx, s.d_out, s.out_cap, out_capacity + 64)) return rc;
+	if (int rc = grow(ctx, s.d_out, out_capacity + 64, kSlotSlack)) return rc;
 	if (int rc = ensure_totals(ctx, s, st)) return rc;
 	if (int rc = run_key_blocks(ctx, s, chunks, pack_bytes, blocks, s.d_out, out_capacity, s.tot_lut, s.tot_res, st)) return rc;
 	uint64_t r[8];
-	CU(cudaMemcpyAsync(r, s.tot_res, 64, cudaMemcpyDeviceToHost, st));
-	CU(cudaStreamSynchronize(st));          // the only synchronisation of the block loop
+	CU(ctx, cudaMemcpyAsync(r, s.tot_res, 64, cudaMemcpyDeviceToHost, st));
+	CU(ctx, cudaStreamSynchronize(st));          // the only synchronisation of the block loop
 	if (r[6]) return fail(ctx, KMCB200_ERR_BIN_FORMAT, "bin format error: the bin does not hold n_rec = %llu k-mers / a pack does not end on a record boundary", (unsigned long long)n_rec);
 	const uint64_t bytes = r[4] * (uint64_t)ob;
 	if (r[5] || bytes > out_capacity) return fail(ctx, KMCB200_ERR_CAPACITY, "out_capacity %llu too small", (unsigned long long)out_capacity);
-	if (bytes) CU(cudaMemcpyAsync(h_out, s.d_out, bytes, cudaMemcpyDeviceToHost, st));
-	CU(cudaMemcpyAsync(h_lut, s.tot_lut, ctx->lut_entries * 8, cudaMemcpyDeviceToHost, st));
-	CU(cudaStreamSynchronize(st));
-	s.last_blocks = (uint32_t)blocks.size();
+	if (bytes) CU(ctx, cudaMemcpyAsync(h_out, s.d_out, bytes, cudaMemcpyDeviceToHost, st));
+	CU(ctx, cudaMemcpyAsync(h_lut, s.tot_lut, ctx->lut_entries * 8, cudaMemcpyDeviceToHost, st));
+	CU(ctx, cudaStreamSynchronize(st));
 	if (out_bytes) *out_bytes = bytes;
 	if (stats) { stats[0] = r[0]; stats[1] = r[1]; stats[2] = r[2]; stats[3] = n_rec; }      // n_total = n_rec (kb_sorter.h:1166)
 	return 0;
@@ -1156,20 +1101,15 @@ int kmcb200_create(const kmcb200_params* prm, kmcb200_ctx** out_ctx)
 	if (prm->lut_prefix_len < 1 || prm->lut_prefix_len >= prm->kmer_len || prm->lut_prefix_len > 15 || (prm->kmer_len - prm->lut_prefix_len) % 4 != 0)
 		return fail(ctx, KMCB200_ERR_INVALID, "lut_prefix_len %u illegal for k=%u: need 1 <= p <= 15, p < k, (k-p) %% 4 == 0 (kmc.h:1434-1469)", prm->lut_prefix_len, prm->kmer_len);
 	if (prm->n_slots < 1 || prm->n_slots > KMCB200_MAX_SLOTS) return fail(ctx, KMCB200_ERR_INVALID, "n_slots %u outside 1..%d", prm->n_slots, KMCB200_MAX_SLOTS);
-	int n_dev = 0;
-	if (cudaGetDeviceCount(&n_dev) != cudaSuccess || n_dev == 0)
-		return fail(ctx, KMCB200_ERR_NO_DEVICE, "no CUDA device visible: kmc_b200 has no CPU fallback");
-	if (prm->device < 0 || prm->device >= n_dev) return fail(ctx, KMCB200_ERR_NO_DEVICE, "device %d not present (%d visible)", prm->device, n_dev);
 	cudaDeviceProp dp;
-	if (cudaGetDeviceProperties(&dp, prm->device) != cudaSuccess) return fail(ctx, KMCB200_ERR_CUDA, "cudaGetDeviceProperties failed");
-	if (dp.major != 9 || dp.minor != 0) return fail(ctx, KMCB200_ERR_NO_DEVICE, "device %d is sm_%d%d; kmc_b200 is built for sm_90a (H100) only", prm->device, dp.major, dp.minor);
+	if (int rc = check_device<kmcb200_ctx>(prm->device, &dp)) return rc;
 
 	ctx = new kmcb200_ctx();
 	ctx->prm = *prm;
 	ctx->words = (int)((prm->kmer_len + 31) / 32);
 	ctx->key_bytes = (prm->kmer_len + 3) / 4;                                  // rec_len, kb_sorter.h:769
 	ctx->suffix_bytes = (prm->kmer_len - prm->lut_prefix_len) / 4;             // kb_sorter.h:1132-1133
-	ctx->counter_bytes = prm->counter_max == 1 ? 0 : std::min(byte_log(prm->cutoff_max), byte_log(prm->counter_max));   // defs.h:154-159
+	ctx->counter_bytes = counter_bytes(prm->cutoff_max, prm->counter_max);
 	ctx->lut_entries = 1ull << (2 * prm->lut_prefix_len);
 	ctx->sm_count = dp.multiProcessorCount;
 	if (const char* e = getenv("KMCB200_SORT")) ctx->use_msd = std::string(e) != "lsd";
@@ -1195,34 +1135,33 @@ int kmcb200_create(const kmcb200_params* prm, kmcb200_ctx** out_ctx)
 	if (const char* e = getenv("KMCB200_LEAF_FILL_PCT")) { const int v = atoi(e); if (v >= 10 && v <= 85) ctx->leaf_fill_pct = (uint32_t)v; }
 	if (const char* e = getenv("KMCB200_LEAF_RATIO0")) { const int v = atoi(e); if (v >= 8 && v <= 256) ctx->leaf_ratio0_q8 = (uint32_t)v; }
 	ctx->slots.resize(prm->n_slots);
-	auto bail = [&](int rc) { std::string e = ctx->err; kmcb200_destroy(ctx); g_create_error = e; return rc; };
-	if (cudaSetDevice(prm->device) != cudaSuccess) { ctx->err = "cudaSetDevice failed"; return bail(KMCB200_ERR_CUDA); }
+	auto bail = [&](int rc) { return create_failed(ctx, kmcb200_destroy, rc); };
+	if (cudaSetDevice(prm->device) != cudaSuccess) return bail(fail(ctx, KMCB200_ERR_CUDA, "cudaSetDevice failed"));
 	if (int rc = DISPATCH_WORDS(ctx, setup_kernels, ctx)) return bail(rc);
 	if (int rc = DISPATCH_WORDS(ctx, setup_leaves, ctx)) return bail(rc);
-	if (cudaFuncSetAttribute(walk_packs_parallel_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kWalkChunk + 32) != cudaSuccess) {
-		ctx->err = "walk_packs_parallel_kernel setup failed"; return bail(KMCB200_ERR_CUDA);
-	}
-	if (cudaStreamCreateWithFlags(&ctx->compute, cudaStreamNonBlocking) != cudaSuccess) { ctx->err = "cudaStreamCreate failed"; return bail(KMCB200_ERR_CUDA); }
+	if (cudaFuncSetAttribute(walk_packs_parallel_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kWalkChunk + 32) != cudaSuccess)
+		return bail(fail(ctx, KMCB200_ERR_CUDA, "walk_packs_parallel_kernel setup failed"));
+	if (cudaStreamCreateWithFlags(&ctx->compute, cudaStreamNonBlocking) != cudaSuccess) return bail(fail(ctx, KMCB200_ERR_CUDA, "cudaStreamCreate failed"));
 	for (auto& s : ctx->slots) {
 		bool ok = cudaStreamCreateWithFlags(&s.stream, cudaStreamNonBlocking) == cudaSuccess;
 		for (cudaEvent_t* e : {&s.ev_h2d, &s.ev_done, &s.ev_walk}) ok = ok && cudaEventCreateWithFlags(e, cudaEventDisableTiming) == cudaSuccess;
-		ok = ok && cudaMalloc(reinterpret_cast<void**>(&s.zero), sizeof(ZeroBlock)) == cudaSuccess;
+		ok = ok && s.zero.alloc(1) == cudaSuccess;
 		ok = ok && cudaMemset(s.zero, 0, sizeof(ZeroBlock)) == cudaSuccess;
-		ok = ok && cudaMalloc(reinterpret_cast<void**>(&s.d_lut), ctx->lut_entries * 8) == cudaSuccess;
-		ok = ok && cudaMalloc(reinterpret_cast<void**>(&s.msd_seg1), 2 * 8) == cudaSuccess;
-		ok = ok && cudaMalloc(reinterpret_cast<void**>(&s.leaf_emit), kMaxLeaves * 4) == cudaSuccess;
-		ok = ok && cudaMalloc(reinterpret_cast<void**>(&s.leaf_off), kMaxLeaves * 8) == cudaSuccess;
-		ok = ok && cudaMalloc(reinterpret_cast<void**>(&s.msd_start2), 257 * 8) == cudaSuccess;
-		ok = ok && cudaMalloc(reinterpret_cast<void**>(&s.msd_start3), (kMaxLeaves + 1) * 8) == cudaSuccess;
-		ok = ok && cudaMalloc(reinterpret_cast<void**>(&s.msd_item_base1), 2 * 4) == cudaSuccess;
-		ok = ok && cudaMalloc(reinterpret_cast<void**>(&s.msd_item_base2), 257 * 4) == cudaSuccess;
-		ok = ok && cudaMalloc(reinterpret_cast<void**>(&s.d_result), 64) == cudaSuccess;
-		ok = ok && cudaHostAlloc(reinterpret_cast<void**>(&s.h_result), 64, cudaHostAllocMapped) == cudaSuccess;
+		ok = ok && s.d_lut.alloc(ctx->lut_entries) == cudaSuccess;
+		ok = ok && s.msd_seg1.alloc(2) == cudaSuccess;
+		ok = ok && s.leaf_emit.alloc(kMaxLeaves) == cudaSuccess;
+		ok = ok && s.leaf_off.alloc(kMaxLeaves) == cudaSuccess;
+		ok = ok && s.msd_start2.alloc(257) == cudaSuccess;
+		ok = ok && s.msd_start3.alloc(kMaxLeaves + 1) == cudaSuccess;
+		ok = ok && s.msd_item_base1.alloc(2) == cudaSuccess;
+		ok = ok && s.msd_item_base2.alloc(257) == cudaSuccess;
+		ok = ok && s.d_result.alloc(8) == cudaSuccess;
+		ok = ok && s.h_result.alloc(8, 0, cudaHostAllocMapped) == cudaSuccess;
 		ok = ok && cudaHostGetDevicePointer(reinterpret_cast<void**>(&s.h_result_dev), s.h_result, 0) == cudaSuccess;
 		for (cudaEvent_t* e : {&s.ev_begin, &s.ev_expand, &s.ev_sort, &s.ev_count, &s.ev_result}) ok = ok && cudaEventCreate(e) == cudaSuccess;
 		for (auto& e : s.ev_pass) ok = ok && cudaEventCreate(&e) == cudaSuccess;
 		for (auto& e : s.ev_pack) ok = ok && cudaEventCreateWithFlags(&e, cudaEventDisableTiming) == cudaSuccess;
-		if (!ok) { ctx->err = std::string("slot allocation failed: ") + cudaGetErrorString(cudaGetLastError()); return bail(KMCB200_ERR_CUDA); }
+		if (!ok) return bail(fail(ctx, KMCB200_ERR_CUDA, "slot allocation failed: %s", cudaGetErrorString(cudaGetLastError())));
 	}
 	*out_ctx = ctx;
 	return KMCB200_OK;
@@ -1234,22 +1173,13 @@ void kmcb200_destroy(kmcb200_ctx* ctx)
 	cudaSetDevice(ctx->prm.device);
 	cudaDeviceSynchronize();
 	for (auto& s : ctx->slots) {
-		for (void* p : {(void*)s.recs_a, (void*)s.recs_b, (void*)s.recs_x, (void*)s.d_bin, (void*)s.d_pack_start, (void*)s.pack_nsk, (void*)s.pack_nk, (void*)s.pack_tbase,
-				 (void*)s.pack_kbase, (void*)s.pack_done, (void*)s.sk_off, (void*)s.sk_kpre, (void*)s.tile_first, (void*)s.tile_pack, (void*)s.tile_desc, (void*)s.zero, (void*)s.desc,
-				 (void*)s.cdesc, (void*)s.d_out, (void*)s.d_lut, (void*)s.d_result, (void*)s.msd_seg1, (void*)s.msd_start2, (void*)s.msd_start3,
-				 (void*)s.msd_item_base1, (void*)s.msd_item_base2, (void*)s.msd_item_seg2, (void*)s.msd_item_lo1, (void*)s.msd_item_cnt1,
-				 (void*)s.msd_cells, (void*)s.msd_cell_scan, (void*)s.msd_block_sums, (void*)s.leaf_tmp, (void*)s.leaf_emit, (void*)s.leaf_off, (void*)s.d_hist12, (void*)s.d_out_counter, (void*)s.tot_lut, (void*)s.tot_res, (void*)s.d_extras, (void*)s.d_pack_rec, (void*)s.d_blk_of_prefix, (void*)s.d_region_start})
-			if (p) cudaFree(p);
-		for (auto p : s.h_pack_start) if (p) cudaFreeHost(p);
 		for (auto e : s.ev_pack) if (e) cudaEventDestroy(e);
-		if (s.h_result) cudaFreeHost(s.h_result);
-		if (s.h_pack_rec) cudaFreeHost(s.h_pack_rec);
 		for (cudaEvent_t e : {s.ev_begin, s.ev_expand, s.ev_sort, s.ev_count, s.ev_result, s.ev_h2d, s.ev_done, s.ev_walk}) if (e) cudaEventDestroy(e);
 		for (auto e : s.ev_pass) if (e) cudaEventDestroy(e);
 		if (s.stream) cudaStreamDestroy(s.stream);
 	}
 	if (ctx->compute) cudaStreamDestroy(ctx->compute);
-	delete ctx;
+	delete ctx;          // (the slots' buffers go with it: the device is idle and still current)
 }
 
 const char* kmcb200_last_error(const kmcb200_ctx* ctx) { return ctx ? ctx->err.c_str() : g_create_error.c_str(); }
@@ -1266,13 +1196,13 @@ int kmcb200_host_alloc(kmcb200_ctx* ctx, uint64_t bytes, void** out_ptr)
 {
 	if (!ctx || !out_ptr) return KMCB200_ERR_INVALID;
 	if (int rc = set_device(ctx)) return rc;
-	CU(cudaHostAlloc(out_ptr, bytes ? bytes : 1, cudaHostAllocDefault));
+	CU(ctx, cudaHostAlloc(out_ptr, bytes ? bytes : 1, cudaHostAllocDefault));
 	return 0;
 }
 int kmcb200_host_free(kmcb200_ctx* ctx, void* ptr)
 {
 	if (!ctx) return KMCB200_ERR_INVALID;
-	if (ptr) CU(cudaFreeHost(ptr));
+	if (ptr) CU(ctx, cudaFreeHost(ptr));
 	return 0;
 }
 
@@ -1311,42 +1241,39 @@ static int submit_bin_impl(kmcb200_ctx* ctx, uint32_t slot, const uint8_t* super
 	if ((size && !superkmers) || !lut || (!out_suffix && out_capacity)) return fail(ctx, KMCB200_ERR_INVALID, "null buffer");
 	if (int rc = set_device(ctx)) return rc;
 	if (n_rec > ctx->max_block_records || size >= 4 * ctx->max_chunk_bytes) {        // oversized: counted key block by key block, synchronously
-		CU(cudaStreamSynchronize(ctx->compute));
+		CU(ctx, cudaStreamSynchronize(ctx->compute));
 		if (int rc = run_oversized_bin(ctx, s, superkmers, size, n_rec, pack_bytes, n_packs, out_suffix, out_capacity, lut, &s.sync_out_bytes, s.sync_stats)) return rc;
 		s.busy = true; s.sync_done = true; s.host_lut = lut;
 		return 0;
 	}
 	cudaStream_t st = s.stream;       // copies
-	if (int rc = ensure(ctx, s.d_bin, s.bin_cap, size + 64)) return rc;
-	if (int rc = ensure(ctx, s.d_out, s.out_cap, out_capacity + 64)) return rc;
-	if (size) CU(cudaMemcpyAsync(s.d_bin, superkmers, size, cudaMemcpyHostToDevice, st));
+	if (int rc = grow(ctx, s.d_bin, size + 64, kSlotSlack)) return rc;
+	if (int rc = grow(ctx, s.d_out, out_capacity + 64, kSlotSlack)) return rc;
+	if (size) CU(ctx, cudaMemcpyAsync(s.d_bin, superkmers, size, cudaMemcpyHostToDevice, st));
 	s.have_extras = false;
 	if (extras && size && n_rec) {          // N4: the length bytes + the first record of every pack travel next to the bin
-		if (int rc = ensure(ctx, s.d_extras, s.extras_cap, n_super_kmers + 64)) return rc;
-		if (int rc = ensure(ctx, s.d_pack_rec, s.pack_rec_cap, (size_t)n_packs + 2)) return rc;
-		if (s.h_pack_rec_cap < (size_t)n_packs + 2) {
-			CU(cudaStreamSynchronize(st));
-			if (s.h_pack_rec) CU(cudaFreeHost(s.h_pack_rec));
-			s.h_pack_rec = nullptr; s.h_pack_rec_cap = 0;
-			CU(cudaHostAlloc(reinterpret_cast<void**>(&s.h_pack_rec), ((size_t)n_packs + 2 + n_packs / 4) * 8, cudaHostAllocDefault));
-			s.h_pack_rec_cap = (size_t)n_packs + 2 + n_packs / 4;
-		} else CU(cudaEventSynchronize(s.ev_h2d));          // (the previous bin's copy out of this staging buffer is done)
+		if (int rc = grow(ctx, s.d_extras, n_super_kmers + 64, kSlotSlack)) return rc;
+		if (int rc = grow(ctx, s.d_pack_rec, (size_t)n_packs + 2, kSlotSlack)) return rc;
+		if (s.h_pack_rec.cap < (size_t)n_packs + 2) {
+			CU(ctx, cudaStreamSynchronize(st));
+			CU(ctx, s.h_pack_rec.alloc((size_t)n_packs + 2 + n_packs / 4));
+		} else CU(ctx, cudaEventSynchronize(s.ev_h2d));          // (the previous bin's copy out of this staging buffer is done)
 		uint64_t acc = 0;
 		for (uint32_t i = 0; i < n_packs; ++i) { s.h_pack_rec[i] = acc; acc += pack_superkmers[i]; }
 		s.h_pack_rec[n_packs] = acc;
 		if (acc != n_super_kmers) return fail(ctx, KMCB200_ERR_BIN_FORMAT, "pack_superkmers add up to %llu records, n_super_kmers is %llu", (unsigned long long)acc, (unsigned long long)n_super_kmers);
-		CU(cudaMemcpyAsync(s.d_extras, extras, n_super_kmers, cudaMemcpyHostToDevice, st));
-		CU(cudaMemcpyAsync(s.d_pack_rec, s.h_pack_rec, ((size_t)n_packs + 1) * 8, cudaMemcpyHostToDevice, st));
+		CU(ctx, cudaMemcpyAsync(s.d_extras, extras, n_super_kmers, cudaMemcpyHostToDevice, st));
+		CU(ctx, cudaMemcpyAsync(s.d_pack_rec, s.h_pack_rec, ((size_t)n_packs + 1) * 8, cudaMemcpyHostToDevice, st));
 		s.have_extras = true;
 	}
 	const bool with_packs = size != 0 && n_rec != 0;
 	if (with_packs) if (int rc = upload_packs(ctx, s, size, pack_bytes, n_packs, st)) return rc;      // on the copy stream, next to the bin
-	CU(cudaEventRecord(s.ev_h2d, st));
-	CU(cudaStreamWaitEvent(ctx->compute, s.ev_h2d, 0));
+	CU(ctx, cudaEventRecord(s.ev_h2d, st));
+	CU(ctx, cudaStreamWaitEvent(ctx->compute, s.ev_h2d, 0));
 	if (int rc = run_bin(ctx, s, s.d_bin, size, n_rec, pack_bytes, n_packs, s.d_out, out_capacity, s.d_lut, s.d_result, ctx->compute, with_packs, s.h_result_dev,
 		st)) return rc;
-	CU(cudaGetLastError());
-	CU(cudaEventRecord(s.ev_result, ctx->compute));
+	CU(ctx, cudaGetLastError());
+	CU(ctx, cudaEventRecord(s.ev_result, ctx->compute));
 	s.busy = true;
 	s.host_out = out_suffix; s.host_out_cap = out_capacity; s.host_lut = lut; s.pending_n_rec = n_rec;
 	return 0;
@@ -1368,7 +1295,7 @@ int kmcb200_wait_bin(kmcb200_ctx* ctx, uint32_t slot, uint64_t* out_bytes, uint6
 		if (stats) for (int i = 0; i < 4; ++i) stats[i] = s.sync_stats[i];
 		return 0;
 	}
-	CU(cudaEventSynchronize(s.ev_result));
+	CU(ctx, cudaEventSynchronize(s.ev_result));
 	const uint64_t* r = s.h_result;
 	if (r[6] & (kErrPackWalk | kErrRecCount)) {
 		cudaStreamSynchronize(s.stream);
@@ -1384,9 +1311,9 @@ int kmcb200_wait_bin(kmcb200_ctx* ctx, uint32_t slot, uint64_t* out_bytes, uint6
 		lut_scan_kernel<<<1, 1024, 0, s.stream>>>(s.d_lut, ctx->lut_entries, s.scan_base);
 		ctx->launches++;
 	}
-	CU(cudaMemcpyAsync(s.host_lut, s.d_lut, ctx->lut_entries * 8, cudaMemcpyDeviceToHost, s.stream));
-	if (bytes) CU(cudaMemcpyAsync(s.host_out, s.d_out, bytes, cudaMemcpyDeviceToHost, s.stream));
-	CU(cudaStreamSynchronize(s.stream));
+	CU(ctx, cudaMemcpyAsync(s.host_lut, s.d_lut, ctx->lut_entries * 8, cudaMemcpyDeviceToHost, s.stream));
+	if (bytes) CU(ctx, cudaMemcpyAsync(s.host_out, s.d_out, bytes, cudaMemcpyDeviceToHost, s.stream));
+	CU(ctx, cudaStreamSynchronize(s.stream));
 	if (out_bytes) *out_bytes = bytes;
 	if (stats) for (int i = 0; i < 4; ++i) stats[i] = r[i];
 	return 0;
@@ -1467,8 +1394,8 @@ int kmcb200_process_bin_multi(kmcb200_ctx* const* ctxs, uint32_t n_ctx, int32_t 
 		if (P.npacks == 0) { P.hist.assign(4096, 0); return 0; }
 		uint64_t dev_bytes = 0;
 		if (int rc = plan_chunks(ctx, P.bytes, pack_bytes + P.pack0, P.npacks, P.chunks, &dev_bytes)) return rc;
-		if (int rc = ensure(ctx, s.d_bin, s.bin_cap, dev_bytes + 64)) return rc;
-		for (const BinChunk& c : P.chunks) CU(cudaMemcpyAsync(s.d_bin + c.dev_off, superkmers + P.byte0 + c.byte0, c.bytes, cudaMemcpyHostToDevice, ctx->compute));
+		if (int rc = grow(ctx, s.d_bin, dev_bytes + 64, kSlotSlack)) return rc;
+		for (const BinChunk& c : P.chunks) CU(ctx, cudaMemcpyAsync(s.d_bin + c.dev_off, superkmers + P.byte0 + c.byte0, c.bytes, cudaMemcpyHostToDevice, ctx->compute));
 		return count_top12(ctx, s, P.chunks, pack_bytes + P.pack0, P.hist, ctx->compute);
 	})) return rc;
 	std::vector<uint64_t> hist(4096, 0);
@@ -1533,24 +1460,24 @@ int kmcb200_process_bin_multi(kmcb200_ctx* const* ctxs, uint32_t n_ctx, int32_t 
 		Part& P = parts[g];
 		if (int rc = set_device(ctx)) return rc;
 		cudaStream_t st = ctx->compute;
-		if (!P.ev_scatter) CU(cudaEventCreateWithFlags(&P.ev_scatter, cudaEventDisableTiming));
+		if (!P.ev_scatter) CU(ctx, cudaEventCreateWithFlags(&P.ev_scatter, cudaEventDisableTiming));
 		uint64_t max_n = 0;
 		for (uint32_t b : P.own) max_n = std::max(max_n, blocks[b].n);
-		if (int rc = ensure(ctx, s.recs_a, s.recs_a_cap, (P.n_share + 2) * rec_bytes)) return rc;                       // the share, scattered by block
-		if (int rc = ensure(ctx, s.recs_x, s.recs_x_cap, (P.n_range + P.own.size() + 2) * rec_bytes)) return rc;       // the range, block after block
-		if (int rc = ensure(ctx, s.recs_b, s.recs_b_cap, (max_n + 2) * rec_bytes)) return rc;                         // one block's scratch
-		if (int rc = ensure(ctx, s.d_out, s.out_cap, P.cap + 64)) return rc;
+		if (int rc = grow(ctx, s.recs_a, (P.n_share + 2) * rec_bytes, kSlotSlack)) return rc;                       // the share, scattered by block
+		if (int rc = grow(ctx, s.recs_x, (P.n_range + P.own.size() + 2) * rec_bytes, kSlotSlack)) return rc;       // the range, block after block
+		if (int rc = grow(ctx, s.recs_b, (max_n + 2) * rec_bytes, kSlotSlack)) return rc;                         // one block's scratch
+		if (int rc = grow(ctx, s.d_out, P.cap + 64, kSlotSlack)) return rc;
 		if (int rc = ensure_totals(ctx, s, st)) return rc;
 		if (P.npacks) {
 			if (int rc = setup_scatter(ctx, s, blocks, P.src_off, st)) return rc;
 			if (int rc = scatter_chunks(ctx, s, P.chunks, pack_bytes + P.pack0, (uint32_t)blocks.size(), s.recs_a, st)) return rc;
 			// (the share must have delivered what its counting pass announced - otherwise the exchange below would copy garbage)
 			std::vector<unsigned long long> got(blocks.size());
-			CU(cudaMemcpyAsync(got.data(), s.d_out_counter, blocks.size() * 8, cudaMemcpyDeviceToHost, st));
-			CU(cudaStreamSynchronize(st));
+			CU(ctx, cudaMemcpyAsync(got.data(), s.d_out_counter, blocks.size() * 8, cudaMemcpyDeviceToHost, st));
+			CU(ctx, cudaStreamSynchronize(st));
 			for (size_t b = 0; b < blocks.size(); ++b) if (got[b] != share_count(g, b)) return fail(ctx, KMCB200_ERR_BIN_FORMAT, "bin format error on GPU %u's share", g);
 		}
-		CU(cudaEventRecord(P.ev_scatter, st));
+		CU(ctx, cudaEventRecord(P.ev_scatter, st));
 		return 0;
 	})) { drop_events(); return rc; }
 	// ---- phase C: the exchange (every GPU pulls its blocks' regions from every GPU), then sort + count block after block, in place
@@ -1565,22 +1492,22 @@ int kmcb200_process_bin_multi(kmcb200_ctx* const* ctxs, uint32_t n_ctx, int32_t 
 			cudaDeviceCanAccessPeer(&can, ctx->prm.device, ctxs[g]->prm.device);
 			if (can) { cudaError_t e = cudaDeviceEnablePeerAccess(ctxs[g]->prm.device, 0); if (e != cudaSuccess) cudaGetLastError(); }      // (already enabled is fine)
 		}
-		for (uint32_t g = 0; g < n_ctx; ++g) CU(cudaStreamWaitEvent(st, parts[g].ev_scatter, 0));
+		for (uint32_t g = 0; g < n_ctx; ++g) CU(ctx, cudaStreamWaitEvent(st, parts[g].ev_scatter, 0));
 		for (size_t i = 0; i < P.own.size(); ++i) {
 			const uint32_t b = P.own[i];
 			uint64_t sub = 0;
 			for (uint32_t g = 0; g < n_ctx; ++g) {
 				const uint64_t c = share_count(g, b);
-				if (c) CU(cudaMemcpyPeerAsync(s.recs_x + (P.dst_off[i] + sub) * rec_bytes, ctx->prm.device,
+				if (c) CU(ctx, cudaMemcpyPeerAsync(s.recs_x + (P.dst_off[i] + sub) * rec_bytes, ctx->prm.device,
 					ctxs[g]->slots[0].recs_a + parts[g].src_off[b] * rec_bytes, ctxs[g]->prm.device, c * rec_bytes, st));
 				sub += c;
 			}
 			if (sub != blocks[b].n) return fail(ctx, KMCB200_ERR_CUDA, "internal error: block %u has %llu records, expected %llu", b, (unsigned long long)sub, (unsigned long long)blocks[b].n);
 			if (int rc = sort_count_block(ctx, s, s.recs_x + P.dst_off[i] * rec_bytes, s.recs_b, blocks[b], s.d_out, P.cap, s.tot_lut, s.tot_res, nullptr, st)) return rc;
 		}
-		CU(cudaMemcpyAsync(P.r, s.tot_res, 64, cudaMemcpyDeviceToHost, st));
-		CU(cudaMemcpyAsync(P.lut.data(), s.tot_lut, ctx->lut_entries * 8, cudaMemcpyDeviceToHost, st));
-		CU(cudaStreamSynchronize(st));
+		CU(ctx, cudaMemcpyAsync(P.r, s.tot_res, 64, cudaMemcpyDeviceToHost, st));
+		CU(ctx, cudaMemcpyAsync(P.lut.data(), s.tot_lut, ctx->lut_entries * 8, cudaMemcpyDeviceToHost, st));
+		CU(ctx, cudaStreamSynchronize(st));
 		return 0;
 	});
 	drop_events();          // (also waits for every GPU: nobody still copies out of a neighbour's scatter buffer)
@@ -1621,13 +1548,13 @@ int kmcb200_sort_records(kmcb200_ctx* ctx, void* recs, void* tmp, uint64_t n, ui
 	const int where = (key_bytes & 1) ? 1 : 0;      // kb_sorter.h:776-779
 	if (n == 0) return where;
 	cudaStream_t st = ctx->compute;
-	if (int rc = ensure(ctx, s.recs_a, s.recs_a_cap, n * rec_bytes)) return rc;
-	if (int rc = ensure(ctx, s.recs_b, s.recs_b_cap, n * rec_bytes)) return rc;
-	CU(cudaMemcpyAsync(s.recs_a, recs, n * rec_bytes, cudaMemcpyHostToDevice, st));
+	if (int rc = grow(ctx, s.recs_a, n * rec_bytes, kSlotSlack)) return rc;
+	if (int rc = grow(ctx, s.recs_b, n * rec_bytes, kSlotSlack)) return rc;
+	CU(ctx, cudaMemcpyAsync(s.recs_a, recs, n * rec_bytes, cudaMemcpyHostToDevice, st));
 	bool in_b = false;
 	if (int rc = DISPATCH_WORDS(ctx, launch_sort, ctx, s, s.recs_a, s.recs_b, n, key_bytes, 8u * key_bytes, (int)kHistNone, 0u, st, &in_b)) return rc;
-	CU(cudaMemcpyAsync(where ? tmp : recs, in_b ? s.recs_b : s.recs_a, n * rec_bytes, cudaMemcpyDeviceToHost, st));
-	CU(cudaStreamSynchronize(st));
+	CU(ctx, cudaMemcpyAsync(where ? tmp : recs, in_b ? s.recs_b : s.recs_a, n * rec_bytes, cudaMemcpyDeviceToHost, st));
+	CU(ctx, cudaStreamSynchronize(st));
 	return where;
 }
 
@@ -1651,14 +1578,14 @@ int kmcb200_dev_expand(kmcb200_ctx* ctx, uint32_t slot, const uint8_t* d_superkm
 	cudaStream_t st = stream ? (cudaStream_t)stream : ctx->compute;
 	if (n_rec == 0) return 0;
 	s.have_extras = false;
-	CU(cudaEventRecord(s.ev_begin, st));
+	CU(ctx, cudaEventRecord(s.ev_begin, st));
 	if (int rc = stage_expand(ctx, s, d_superkmers, size, n_rec, pack_bytes, n_packs, d_recs, st)) return rc;
 	if (d_result) {
 		if (int rc = zero_async(ctx, d_result, 64, st)) return rc;
 		finish_result_kernel<<<1, 32, 0, st>>>(d_result, n_rec, s.zero->status, nullptr, nullptr);
 		ctx->launches++;
 	}
-	CU(cudaEventRecord(s.ev_expand, st));
+	CU(ctx, cudaEventRecord(s.ev_expand, st));
 	s.ran_expand = true; s.ran_sort = s.ran_count = false;
 	return 0;
 }
@@ -1672,10 +1599,10 @@ int kmcb200_dev_sort(kmcb200_ctx* ctx, uint32_t slot, void* d_recs, void* d_tmp,
 	cudaStream_t st = stream ? (cudaStream_t)stream : ctx->compute;
 	const int where = (key_bytes & 1) ? 1 : 0;
 	if (n == 0) return where;
-	if (!hist_ready) CU(cudaEventRecord(s.ev_expand, st));
+	if (!hist_ready) CU(ctx, cudaEventRecord(s.ev_expand, st));
 	bool in_b = false;
 	if (int rc = DISPATCH_WORDS(ctx, launch_sort, ctx, s, d_recs, d_tmp, n, key_bytes, hist_ready ? 2u * ctx->prm.kmer_len : 8u * key_bytes, hist_ready ? s.hist_mode : (int)kHistNone, s.last_n_packs, st, &in_b)) return rc;
-	CU(cudaEventRecord(s.ev_sort, st));
+	CU(ctx, cudaEventRecord(s.ev_sort, st));
 	s.ran_sort = true; s.ran_count = false;
 	if (!hist_ready) s.ran_expand = false;
 	return in_b ? 1 : 0;
@@ -1688,11 +1615,11 @@ int kmcb200_dev_count(kmcb200_ctx* ctx, uint32_t slot, const void* d_sorted, uin
 	if (int rc = set_device(ctx)) return rc;
 	Slot& s = ctx->slots[slot];
 	cudaStream_t st = stream ? (cudaStream_t)stream : ctx->compute;
-	CU(cudaEventRecord(s.ev_sort, st));
+	CU(ctx, cudaEventRecord(s.ev_sort, st));
 	if (int rc = stage_count(ctx, s, d_sorted, n, d_out, out_capacity, d_lut, d_result, st)) return rc;
 	finish_result_kernel<<<1, 32, 0, st>>>(d_result, n, nullptr, nullptr, nullptr);
 	ctx->launches++;
-	CU(cudaEventRecord(s.ev_count, st));
+	CU(ctx, cudaEventRecord(s.ev_count, st));
 	s.ran_count = true; s.ran_expand = false; s.ran_sort = false;
 	return 0;
 }
@@ -1704,15 +1631,15 @@ int kmcb200_stage_times(kmcb200_ctx* ctx, uint32_t slot, float* ms, uint32_t cap
 	if (int rc = set_device(ctx)) return rc;
 	Slot& s = ctx->slots[slot];
 	for (uint32_t i = 0; i < capacity; ++i) ms[i] = 0.f;
-	if (s.ran_count) CU(cudaEventSynchronize(s.ev_count));
-	else if (s.ran_sort) CU(cudaEventSynchronize(s.ev_sort));
-	else if (s.ran_expand) CU(cudaEventSynchronize(s.ev_expand));
-	if (s.ran_expand) CU(cudaEventElapsedTime(&ms[0], s.ev_begin, s.ev_expand));
+	if (s.ran_count) CU(ctx, cudaEventSynchronize(s.ev_count));
+	else if (s.ran_sort) CU(ctx, cudaEventSynchronize(s.ev_sort));
+	else if (s.ran_expand) CU(ctx, cudaEventSynchronize(s.ev_expand));
+	if (s.ran_expand) CU(ctx, cudaEventElapsedTime(&ms[0], s.ev_begin, s.ev_expand));
 	if (s.ran_sort) {
-		CU(cudaEventElapsedTime(&ms[1], s.ev_expand, s.ev_sort));
-		for (int p = 0; p < s.n_passes_run && 3 + p < (int)capacity; ++p) CU(cudaEventElapsedTime(&ms[3 + p], s.ev_pass[p], s.ev_pass[p + 1]));
+		CU(ctx, cudaEventElapsedTime(&ms[1], s.ev_expand, s.ev_sort));
+		for (int p = 0; p < s.n_passes_run && 3 + p < (int)capacity; ++p) CU(ctx, cudaEventElapsedTime(&ms[3 + p], s.ev_pass[p], s.ev_pass[p + 1]));
 	}
-	if (s.ran_count) CU(cudaEventElapsedTime(&ms[2], s.ev_sort, s.ev_count));
+	if (s.ran_count) CU(ctx, cudaEventElapsedTime(&ms[2], s.ev_sort, s.ev_count));
 	return s.ran_sort ? s.n_passes_run : 0;
 }
 

@@ -257,6 +257,13 @@ STAGE1_CASES = {
     "k55_p9_ndense_b": (104, "n_dense", 2000, 200, 55, ("-p9", "-ci1", "-b")),
     "k96_p7_canon": (105, "short", 2000, 250, 96, ("-p7", "-ci1", "-cs65535")),
     "k17_p7_ndense": (106, "n_dense", 3000, 150, 17, ("-p7", "-ci2")),
+    # k mod 32 = 29 / 30: stage 2 sorts (k+x)-mers with max_x = 2 / 1, so the (k+x)-mer counts of stage 1 decide the bin order
+    "k29_p9_canon": (107, "short", 3000, 150, 29, ("-p9", "-ci1")),
+    "k30_p6_b": (108, "short", 3000, 150, 30, ("-p6", "-ci1", "-b")),
+    "k30_p11_lowcomplex": (109, "low_complexity", 300, 1500, 30, ("-p11", "-ci2", "-cs65535")),
+    "k61_p8_ndense_b": (110, "n_dense", 2000, 200, 61, ("-p8", "-ci1", "-b")),
+    "k62_p8_canon": (111, "short", 2000, 200, 62, ("-p8", "-ci1")),
+    "k93_p10_b": (112, "short", 2000, 250, 93, ("-p10", "-ci1", "-b")),
 }
 
 

@@ -1,7 +1,8 @@
-"""The level 1 of a bin of one-word records on the MSD path: a counting expansion (expand_kernel<kExpandCells>) and an expansion that writes
-every k-mer straight into its level-1 bucket (expand_kernel<kExpandPartition>, the `expand_scatter_L1` interval).  Each case is compared
-with the sequence that writes the records in tile order and partitions them afterwards (dev_expand -> dev_sort(hist_ready) -> dev_count,
-which keeps expand_kernel<kExpandAll> + msd_partition_kernel) and with the oracle: the same payload, LUT and result words."""
+"""The level 1 of a bin of one-word records on the MSD path: the pack walk counts the level-1 digit of every k-mer into 256 totals, and the
+one expansion of the bin writes every k-mer straight into its level-1 bucket (expand_kernel<kExpandPartition>, the `expand_scatter_L1`
+interval).  Each case is compared with the sequence that writes the records in tile order and partitions them afterwards (dev_expand ->
+dev_sort(hist_ready) -> dev_count, which keeps expand_kernel<kExpandAll> + msd_partition_kernel) and with the oracle: the same payload,
+LUT and result words."""
 import numpy as np
 import pytest
 
@@ -139,8 +140,8 @@ def test_skewed_bin_takes_the_lsd_fallback(oracle):
 
 @pytest.mark.parametrize("delta", [1, -1])
 def test_malformed_bin_stops_on_the_device(oracle, delta):
-    """n_rec one more / one less than the bin holds: the pack scan stops the bin before the counting expansion writes a cell, the
-    partition expansion and everything behind it return at once, nothing is emitted.  A good bin on the same context is then right."""
+    """n_rec one more / one less than the bin holds: the pack scan stops the bin, the partition expansion and everything behind it
+    return at once, nothing is emitted.  A good bin on the same context is then right."""
     import kmc_b200
     p = Params(k=31, cutoff_min=2, lut_prefix_len=7)
     b = fast_bin(5, 31, 300_000)

@@ -364,6 +364,46 @@ int kmcb200_smallk_emit(kmcb200_smallk* h, uint8_t* suffix, uint64_t capacity, u
 int kmcb200_smallk_write_db(kmcb200_smallk* h, const char* path_prefix, uint32_t cutoff_min, uint64_t cutoff_max, uint64_t counter_max,
 	uint64_t* totals);
 
+/* ---- histogram estimation (KMC's CntHashEstimator, kmc_core/libs/ntHash/ntHashWrapper.h:97-454: `kmc -e`, `kmc --opt-out-size`) --------
+ * The batch format is kmcb200_split's; every k-mer of ACGT only is hashed with canonical ntHash, h = min(fh, rh) (64 bits), and sampled:
+ * counters[0][h mod 2^27] += 1 when h >> (63 - s) == 1, counters[1][h mod 2^27] += 1 when h >> (64 - s) == 2^(s-1) - 1 (two tables of
+ * 2^27 uint32).  The counters are a function of the multiset of k-mers alone, and add up over calls until reset.
+ *   histogram  max_occ = min(max(largest counter, 2), 65536); hist[0..max_occ] the reference's EstimateHistogram of the two tables'
+ *              histograms of min(65536, counter): hist[i] estimates the number of distinct k-mers that occur i times, hist[0] = 0.  The
+ *              recursion, O(max_occ^2) in double, runs on the host in the reference's order of operations.
+ * `kmc` takes s = 7, or 11 when the input files hold at least 5 * 10^10 bytes (kmc.h:1118-1121).
+ * Work: 1 launch per add, 1 per histogram (one synchronisation).  Workspace: the batch (max_batch_bytes, host path) and 1 GiB of counters. */
+#define KMCB200_ESTIMATE_MAX_KMER_LEN 256
+typedef struct kmcb200_estimator kmcb200_estimator;
+typedef struct {
+	uint32_t kmer_len;                    /* 1..KMCB200_ESTIMATE_MAX_KMER_LEN */
+	uint32_t s;                           /* 7 or 11 */
+	int32_t device;                       /* CUDA ordinal */
+	uint32_t reserved;                    /* 0 */
+	uint64_t max_batch_bytes;             /* largest batch one call accepts (1..KMCB200_SPLIT_MAX_BATCH) */
+} kmcb200_estimator_params;
+/* KMCB200_ERR_INVALID for a bad parameter, KMCB200_ERR_NO_DEVICE without an sm_90 device (no CPU fallback).  The counters start at 0. */
+int kmcb200_estimator_create(const kmcb200_estimator_params* params, kmcb200_estimator** out);
+void kmcb200_estimator_destroy(kmcb200_estimator* h);
+/* message of the last failure on this handle (or of the last failed create when h == NULL) */
+const char* kmcb200_estimator_last_error(const kmcb200_estimator* h);
+/* Number of kernels this handle has launched so far. */
+uint64_t kmcb200_estimator_kernel_launches(const kmcb200_estimator* h);
+/* Host batch: copied in, hashed; returns when the batch buffer may be reused.  A batch over max_batch_bytes: KMCB200_ERR_INVALID. */
+int kmcb200_estimator_add(kmcb200_estimator* h, const uint8_t* seq, uint64_t bytes);
+/* Device twin: d_seq in HBM, queued on `stream` (a cudaStream_t; NULL = the legacy default stream) after the handle's earlier work. */
+int kmcb200_dev_estimator_add(kmcb200_estimator* h, const uint8_t* d_seq, uint64_t bytes, void* stream);
+/* kmcb200_estimator_add of a raw FASTQ / FASTA chunk parsed on the GPU straight into the handle's batch buffer (see kmcb200_fastx_parse for
+ * is_final and *consumed; *seq_bytes and *n_records, which may be NULL, receive the batch's length and the records parsed).  bytes + 1 >
+ * max_batch_bytes: KMCB200_ERR_INVALID.  Errors are reported on the estimator. */
+int kmcb200_estimator_add_fastx(kmcb200_estimator* h, kmcb200_fastx* p, const uint8_t* raw, uint64_t bytes, int is_final, uint64_t* consumed,
+	uint64_t* seq_bytes, uint64_t* n_records);
+/* counters[2 * 2^27] (host): table 0, then table 1, after every call queued so far, device twin included. */
+int kmcb200_estimator_read(kmcb200_estimator* h, uint32_t* counters);
+/* *n = max_occ + 1 and hist[0, *n) the estimate of the current counters.  capacity < *n: KMCB200_ERR_CAPACITY, *n set, hist not written. */
+int kmcb200_estimator_histogram(kmcb200_estimator* h, uint64_t* hist, uint64_t capacity, uint64_t* n);
+int kmcb200_estimator_reset(kmcb200_estimator* h);
+
 /* ---- seam #1: sort host records ------------------------------------------------------------------
  * Contract of SortFunction (raduls.h:19-20, kb_sorter.h:775-779): n records of rec_bytes (multiple of 8,
  * CKmer<SIZE> images) sorted ascending on bytes key_bytes-1..0; the result is left in `tmp` when key_bytes

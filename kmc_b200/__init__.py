@@ -47,6 +47,10 @@ class _SmallKParams(C.Structure):
     _fields_ = [("kmer_len", C.c_uint32), ("both_strands", C.c_uint32), ("device", C.c_int32), ("reserved", C.c_uint32), ("max_batch_bytes", C.c_uint64)]
 
 
+class _EstimatorParams(C.Structure):
+    _fields_ = [("kmer_len", C.c_uint32), ("s", C.c_uint32), ("device", C.c_int32), ("reserved", C.c_uint32), ("max_batch_bytes", C.c_uint64)]
+
+
 class _FastxParams(C.Structure):
     _fields_ = [("device", C.c_int32), ("format", C.c_uint32), ("max_chunk_bytes", C.c_uint64)]
 
@@ -72,6 +76,9 @@ EXPORTS = [
     "kmcb200_smallk_create", "kmcb200_smallk_destroy", "kmcb200_smallk_last_error", "kmcb200_smallk_kernel_launches", "kmcb200_smallk_add",
     "kmcb200_dev_smallk_add", "kmcb200_smallk_add_fastx", "kmcb200_smallk_read", "kmcb200_smallk_reset", "kmcb200_smallk_finish",
     "kmcb200_smallk_emit", "kmcb200_smallk_write_db",
+    "kmcb200_estimator_create", "kmcb200_estimator_destroy", "kmcb200_estimator_last_error", "kmcb200_estimator_kernel_launches",
+    "kmcb200_estimator_add", "kmcb200_dev_estimator_add", "kmcb200_estimator_add_fastx", "kmcb200_estimator_read",
+    "kmcb200_estimator_histogram", "kmcb200_estimator_reset",
 ]
 
 FASTQ, FASTA = 1, 2                                                     # KMCB200_FASTQ / KMCB200_FASTA
@@ -177,6 +184,19 @@ def load_library(build_if_needed=True):
     L.kmcb200_smallk_finish.argtypes = [vp, u32, u64, u64, C.POINTER(u32), C.POINTER(u32), C.POINTER(u64), vp]
     L.kmcb200_smallk_emit.argtypes = [vp, vp, u64, vp]
     L.kmcb200_smallk_write_db.argtypes = [vp, C.c_char_p, u32, u64, u64, vp]
+    L.kmcb200_estimator_create.argtypes = [C.POINTER(_EstimatorParams), C.POINTER(vp)]
+    L.kmcb200_estimator_destroy.argtypes = [vp]
+    L.kmcb200_estimator_destroy.restype = None
+    L.kmcb200_estimator_last_error.argtypes = [vp]
+    L.kmcb200_estimator_last_error.restype = C.c_char_p
+    L.kmcb200_estimator_kernel_launches.argtypes = [vp]
+    L.kmcb200_estimator_kernel_launches.restype = u64
+    L.kmcb200_estimator_add.argtypes = [vp, vp, u64]
+    L.kmcb200_dev_estimator_add.argtypes = [vp, vp, u64, vp]
+    L.kmcb200_estimator_add_fastx.argtypes = [vp, vp, vp, u64, C.c_int, C.POINTER(u64), C.POINTER(u64), C.POINTER(u64)]
+    L.kmcb200_estimator_read.argtypes = [vp, vp]
+    L.kmcb200_estimator_histogram.argtypes = [vp, vp, u64, C.POINTER(u64)]
+    L.kmcb200_estimator_reset.argtypes = [vp]
     _lib = L
     return L
 
@@ -590,6 +610,58 @@ class SmallKCounter(_Handle):
         self._check(self.lib.kmcb200_smallk_write_db(self._h, path_prefix.encode(), cutoff_min, min(int(cutoff_max), (1 << 64) - 1),
                                                      min(int(counter_max), (1 << 64) - 1), tot))
         return tuple(int(x) for x in tot)
+
+
+class HistogramEstimator(_Handle):
+    """KMC's histogram estimator on one GPU (kmcb200_estimator_*), what `kmc -e` and `kmc --opt-out-size` run (CntHashEstimator,
+    kmc_core/libs/ntHash/ntHashWrapper.h): the canonical ntHash of every k-mer (1 <= k <= 256) of the batches, sampled into two tables of
+    2^27 uint32 counters with s = 7 or 11; histogram() is the reference's estimate of the k-mer count histogram.  Batches as for Splitter;
+    the counters add up until reset().  The handle holds 1 GiB of counters on the device."""
+    _prefix = "kmcb200_estimator"
+    TABLE = 1 << 27
+
+    def __init__(self, kmer_len, s=7, device=0, max_batch_bytes=1 << 26):
+        self.kmer_len, self.s, self.max_batch_bytes = kmer_len, s, max_batch_bytes
+        p = _EstimatorParams(kmer_len, s, device, 0, max_batch_bytes)
+        self._open(C.byref(p))
+
+    def kernel_launches(self):
+        return int(self.lib.kmcb200_estimator_kernel_launches(self._h))
+
+    def add(self, batch):
+        seq = _as_u8(batch)
+        self._check(self.lib.kmcb200_estimator_add(self._h, seq.ctypes.data, seq.size))
+
+    def dev_add(self, d_seq, nbytes, stream=None):
+        """kmcb200_dev_estimator_add: d_seq a device pointer (int or a tensor's data_ptr()), queued on `stream` (a cudaStream_t)."""
+        self._check(self.lib.kmcb200_dev_estimator_add(self._h, d_seq, nbytes, stream))
+
+    def add_fastx(self, parser, raw, is_final=True):
+        """kmcb200_estimator_add_fastx: a raw FASTQ / FASTA chunk parsed on the GPU by `parser` and hashed.  Returns `consumed`, the bytes
+        parsed (the caller carries the rest into its next chunk); the batch's length and the records parsed are left in last_seq_bytes and
+        last_records."""
+        a = _as_u8(raw)
+        consumed, seq_bytes, recs = C.c_uint64(0), C.c_uint64(0), C.c_uint64(0)
+        self._check(self.lib.kmcb200_estimator_add_fastx(self._h, parser._h, a.ctypes.data, a.size, int(bool(is_final)), C.byref(consumed),
+                                                         C.byref(seq_bytes), C.byref(recs)))
+        self.last_seq_bytes, self.last_records = int(seq_bytes.value), int(recs.value)
+        return int(consumed.value)
+
+    def read(self):
+        """uint32[2, 2^27]: the two counter tables."""
+        out = np.zeros((2, self.TABLE), dtype=np.uint32)
+        self._check(self.lib.kmcb200_estimator_read(self._h, out.ctypes.data))
+        return out
+
+    def histogram(self):
+        """uint64[max_occ + 1]: entry i estimates the distinct k-mers that occur i times (entry 0 is 0), as `kmc -e` writes it."""
+        out = np.zeros(65537, dtype=np.uint64)
+        n = C.c_uint64(0)
+        self._check(self.lib.kmcb200_estimator_histogram(self._h, out.ctypes.data, out.size, C.byref(n)))
+        return out[:n.value].copy()
+
+    def reset(self):
+        self._check(self.lib.kmcb200_estimator_reset(self._h))
 
 
 def _as_u8(raw):

@@ -9,8 +9,9 @@ DEPS = sorted(os.path.join(HERE, "csrc", f) for f in os.listdir(os.path.join(HER
     os.path.join(os.path.dirname(HERE), "include", "kmc_b200.h")]
 OUT = os.path.join(HERE, "libkmc_b200.so")
 NVCC = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
+# -ffp-contract=off: the host code rounds every product and sum on its own, as the reference's CPU code does (the estimator's recursion)
 FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-O3", "-std=c++17", "--shared", "-Xcompiler", "-fPIC",
-         "-Xcompiler", "-fvisibility=default"]
+         "-Xcompiler", "-fvisibility=default", "-Xcompiler", "-ffp-contract=off"]
 
 
 def needs_build():

@@ -16,6 +16,7 @@
 #include "split.cuh"
 #include "fastx.cuh"
 #include "small_k.cuh"
+#include "estimate.cuh"
 
 #include <cmath>
 #include <cstddef>
@@ -1661,3 +1662,4 @@ int kmcb200_stage_names(kmcb200_ctx* ctx, uint32_t slot, char* buf, uint32_t cap
 #include "stage0.inl"
 #include "fastx.inl"
 #include "small_k.inl"
+#include "estimate.inl"

@@ -25,6 +25,12 @@ Small k (k <= 13, `count_reads_small_k`, `--small-k`): KMC's small-k mode.  Ever
 GPU (kmc_b200.SmallKCounter), with no bins, and the database is written in the KMC1 format the reference writes in that mode (version word
 0, no signature map), byte for byte `kmc -kK`'s when the reference takes its small-k path.  count_reads takes this path by itself where the
 bin path cannot run, k <= signature_len.
+
+Histogram estimation (`estimate_histogram`, `-e`): KMC's ntHash estimator (`kmc -e`) on the GPU (kmc_b200.HistogramEstimator), for
+1 <= k <= 256; the file `-e` writes is the reference's, "i<TAB>count" per line.  count_reads(opt_out_size=True) runs the same estimator over
+the chunks it splits and picks the LUT prefix length from the estimated number of counted k-mers, as `kmc --opt-out-size` does.
+
+    python -m kmc_b200.reads -e -k31 reads.fq hist.txt
 """
 import argparse
 import json
@@ -37,8 +43,8 @@ import time
 
 import numpy as np
 
-from . import DbWriter, FASTA, FASTQ, FastxParser, KmcB200Error, ERR_INVALID, SignatureStats, SmallKCounter, Splitter, Stage2Context, \
-    Stage2Params, signature_map as _signature_map, stage2_bin_order
+from . import DbWriter, FASTA, FASTQ, FastxParser, HistogramEstimator, KmcB200Error, ERR_INVALID, SignatureStats, SmallKCounter, Splitter, \
+    Stage2Context, Stage2Params, signature_map as _signature_map, stage2_bin_order
 
 _NL, _GT, _AT = 10, ord(">"), ord("@")
 STATS_SAMPLE_BYTES = 1 << 28                                            # STATS_FASTQ_SIZE (kmc_core/defs.h)
@@ -275,6 +281,86 @@ def signature_sample_counts(paths, k, signature_len, batch_bytes=1 << 26, device
 
 
 SMALL_K_MAX = 13
+ESTIMATE_MAX_K = 256
+ESTIMATE_LARGE_INPUT = 50_000_000_000                                   # kmc.h:1118-1121: s = 11 from this many input bytes on
+
+
+def estimate_s(paths):
+    """The reference's sampling exponent for these inputs: 7, or 11 when the files hold at least 5 * 10^10 bytes."""
+    return 11 if sum(os.path.getsize(p) for p in paths) >= ESTIMATE_LARGE_INPUT else 7
+
+
+def n_records(data):
+    """FASTQ records or FASTA headers in a chunk of whole records: the reads CSplitter::GetSeq counts (splitter.cpp:68-417)."""
+    a = _as_array(data)
+    if a.size == 0:
+        return 0
+    starts = np.concatenate([[0], np.flatnonzero(a[:-1] == _NL) + 1])
+    if fastx_format(a) == FASTA:
+        return int(np.count_nonzero(a[starts] == _GT))
+    return (int(np.count_nonzero(a[starts] != _NL)) + 3) // 4
+
+
+def _as_array(data):
+    return np.frombuffer(data, dtype=np.uint8) if isinstance(data, (bytes, bytearray, memoryview)) else np.asarray(data, dtype=np.uint8)
+
+
+def kmc_lut_prefix_len(k, n_est_kmers, n_bins):
+    """The LUT prefix length `kmc` picks for a bin database (kmc.h:1432-1468): lp of 2..15 with (k - lp) % 4 == 0 (uint32 arithmetic)
+    of least n_est * (k - lp) / 4 + n_bins * 4^lp * 8 (uint64), the first on a tie.  n_est is 4 * n_reads, or with --opt-out-size the
+    estimated number of counted k-mers."""
+    m64 = (1 << 64) - 1
+    best, best_mem = 0, 1 << 62
+    for lp in range(2, 16):
+        suffix = (k - lp) & 0xFFFFFFFF
+        if suffix % 4:
+            continue
+        mem = (((n_est_kmers * suffix) & m64) // 4 + n_bins * (1 << (2 * lp)) * 8) & m64
+        if mem < best_mem:
+            best, best_mem = lp, mem
+    return best
+
+
+def estimated_counted_kmers(hist, cutoff_min, cutoff_max):
+    """kmc.h:1441-1447: the estimate summed over cutoff_min .. min(cutoff_max + 1, len) - 1."""
+    end = min(int(cutoff_max) + 1, len(hist))
+    return int(sum(int(v) for v in hist[int(cutoff_min):end])) & ((1 << 64) - 1)
+
+
+def estimate_histogram(paths, k, s=None, batch_bytes=1 << 26, device=0, parse="host"):
+    """`kmc -e` on one GPU: the reference's ntHash estimate of the k-mer count histogram of the files (canonical k-mers, 1 <= k <= 256),
+    uint64[max_occ + 1] with entry 0 = 0.  s: 7 or 11, default the reference's rule on the input size (estimate_s).  parse as for
+    count_reads."""
+    if parse not in ("host", "gpu"):
+        raise KmcB200Error(ERR_INVALID, "parse must be 'host' or 'gpu', not %r" % (parse,))
+    est = HistogramEstimator(k, estimate_s(paths) if s is None else s, device, max_batch_bytes=batch_bytes)
+    parsers = _Parsers(device, batch_bytes - 1) if parse == "gpu" else None
+    try:
+        for path in paths:
+            if parsers is not None:
+                with _RawChunks(path, batch_bytes - 1) as chunks:
+                    parser = None
+                    for chunk, final in chunks:
+                        parser = parser or parsers(chunk)
+                        chunks.consumed(est.add_fastx(parser, chunk, final))
+                continue
+            with open(path, "rb") as f:
+                data = f.read()
+            if not data:
+                continue
+            for batch in batches(sequences_to_batch(data), batch_bytes):
+                est.add(batch)
+        return est.histogram()
+    finally:
+        if parsers is not None:
+            parsers.close()
+        est.close()
+
+
+def write_histogram(path, hist):
+    """The file `kmc -e` writes (kmc_CLI/kmc.cpp:308-321): "i\tcount\n" for i = 1 .. len - 1."""
+    with open(path, "w") as f:
+        f.write("".join("%d\t%d\n" % (i, int(v)) for i, v in enumerate(hist) if i))
 
 
 def count_reads_small_k(paths, out_prefix, k, cutoff_min=2, cutoff_max=1_000_000_000, counter_max=255, both_strands=True, batch_bytes=1 << 26,
@@ -325,8 +411,8 @@ def count_reads_small_k(paths, out_prefix, k, cutoff_min=2, cutoff_max=1_000_000
             "lut_prefix_len": lp}
 
 
-def count_reads(paths, out_prefix, k, signature_len, signature_map, lut_prefix_len, cutoff_min=2, cutoff_max=1_000_000_000, counter_max=255,
-                both_strands=True, batch_bytes=1 << 26, device=0, n_bins=None, parse="host", small_k=None):
+def count_reads(paths, out_prefix, k, signature_len, signature_map, lut_prefix_len=None, cutoff_min=2, cutoff_max=1_000_000_000, counter_max=255,
+                both_strands=True, batch_bytes=1 << 26, device=0, n_bins=None, parse="host", small_k=None, opt_out_size=False):
     """KMC's stages on one GPU in RAM mode: every batch of every file is split on the GPU and the bin fragments stay in host memory;
     then bin by bin, stage 2 and the database writer.  Returns the writer's totals and the split's counts.
     With a signature_map: the bins are written in bin-id order, bin b's signatures (the map's preimage of b) go into .kmc_pre, and n_bins
@@ -338,10 +424,20 @@ def count_reads(paths, out_prefix, k, signature_len, signature_map, lut_prefix_l
     parses them on the GPU (kmc_b200.FastxParser, see the module docstring); the files and counts are the same either way.
     small_k: None takes the small-k path (count_reads_small_k) where the bin path cannot run, k <= signature_len; True takes it for any
     k <= 13, as `kmc` does; False keeps the bin path.  On the small-k path signature_len, signature_map, n_bins and lut_prefix_len are not
-    used, and the result also holds the lut_prefix_len the path chose."""
+    used, and the result also holds the lut_prefix_len the path chose.
+    lut_prefix_len=None picks it as `kmc` does (kmc_lut_prefix_len): from 4 * n_reads, the records of the input (FASTQ records, FASTA
+    headers), or with opt_out_size=True from the estimate of the counted k-mers, which the histogram estimator (HistogramEstimator, s by
+    estimate_s) computes over the same batches as the split, as `kmc --opt-out-size` does.  opt_out_size needs canonical k-mers and the
+    bin path.  The result holds n_reads and the lut_prefix_len used."""
     if parse not in ("host", "gpu"):
         raise KmcB200Error(ERR_INVALID, "parse must be 'host' or 'gpu', not %r" % (parse,))
+    if opt_out_size and not both_strands:
+        raise KmcB200Error(ERR_INVALID, "k-mer histogram estimation possible only for canonical k-mers")
+    if opt_out_size and lut_prefix_len is not None:
+        raise KmcB200Error(ERR_INVALID, "opt_out_size chooses the LUT prefix length: give lut_prefix_len=None")
     if small_k or (small_k is None and k <= signature_len):
+        if opt_out_size:
+            raise KmcB200Error(ERR_INVALID, "histogram estimation is not supported on the small-k path, as in kmc")
         return count_reads_small_k(paths, out_prefix, k, cutoff_min, cutoff_max, counter_max, both_strands, batch_bytes, device, parse)
     t0 = time.perf_counter()
     if signature_map is None:
@@ -357,8 +453,9 @@ def count_reads(paths, out_prefix, k, signature_len, signature_map, lut_prefix_l
     sp = Splitter(k, signature_len, sig_map, n_bins, device, max_batch_bytes=batch_bytes)
     if mapper is not None:
         sp.count_kxmers(both_strands)
+    est = HistogramEstimator(k, estimate_s(paths), device, max_batch_bytes=batch_bytes) if opt_out_size else None
     parts = [[] for _ in range(n_bins)]
-    n_super = n_kmers = n_bases = 0
+    n_super = n_kmers = n_bases = n_reads = 0
     read_s = 0.0
 
     def keep(out, packs, frags):
@@ -378,6 +475,11 @@ def count_reads(paths, out_prefix, k, signature_len, signature_map, lut_prefix_l
                     for chunk, final in chunks:
                         parser = parser or parsers(chunk)
                         out, packs, frags, used, nseq = sp.split_fastx(parser, chunk, final)
+                        if est is not None:
+                            est.add_fastx(parser, chunk[:used], True)
+                            n_reads += est.last_records
+                        else:
+                            n_reads += n_records(chunk[:used])
                         chunks.consumed(used)
                         n_bases += nseq
                         keep(out, packs, frags)
@@ -387,15 +489,23 @@ def count_reads(paths, out_prefix, k, signature_len, signature_map, lut_prefix_l
             with open(path, "rb") as f:
                 data = f.read()
             read_s += time.perf_counter() - t
+            n_reads += n_records(data)
             seq = sequences_to_batch(data)
             del data
             for batch in batches(seq, batch_bytes):
                 out, packs, frags = sp.split_raw(batch)
+                if est is not None:
+                    est.add(batch)
                 n_bases += batch.size
                 keep(out, packs, frags)
+        if lut_prefix_len is None:
+            n_est = estimated_counted_kmers(est.histogram(), cutoff_min, cutoff_max) if est is not None else 4 * n_reads
+            lut_prefix_len = kmc_lut_prefix_len(k, n_est, n_bins)
     finally:
         if parsers is not None:
             parsers.close()
+        if est is not None:                                             # before the stage-2 context sizes itself from free HBM
+            est.close()
     if mapper is None:
         file_order = np.arange(n_bins)
         order = np.argsort(sig_map, kind="stable")
@@ -430,7 +540,8 @@ def count_reads(paths, out_prefix, k, signature_len, signature_map, lut_prefix_l
     ctx.close()
     t2 = time.perf_counter()
     return {"n_unique": totals[0], "n_cutoff_min": totals[1], "n_cutoff_max": totals[2], "n_total": totals[3], "n_super_kmers": n_super,
-            "n_kmers": n_kmers, "n_bases": n_bases, "stats_s": t_stats, "split_s": t1 - t0 - t_stats, "stage2_s": t2 - t1, "read_s": read_s}
+            "n_kmers": n_kmers, "n_bases": n_bases, "stats_s": t_stats, "split_s": t1 - t0 - t_stats, "stage2_s": t2 - t1, "read_s": read_s,
+            "n_reads": n_reads, "lut_prefix_len": lut_prefix_len}
 
 
 def main(argv=None):
@@ -442,6 +553,9 @@ def main(argv=None):
     ap.add_argument("--map", help=".npy file with the 4^p + 1 map entries (default: chosen from the reads, as KMC does)")
     ap.add_argument("--map-from", help="take p and the map from this .kmc_pre")
     ap.add_argument("--lut-prefix-len", type=int, default=None, help="default: the smallest of 7, 3, 11, ... with (k - p) %% 4 == 0")
+    ap.add_argument("--opt-out-size", action="store_true",
+                    help="pick the LUT prefix length from the estimated number of counted k-mers, as kmc --opt-out-size does")
+    ap.add_argument("-e", action="store_true", help="write the estimated k-mer count histogram to the last argument instead of counting (kmc -e)")
     ap.add_argument("--ci", type=int, default=2)
     ap.add_argument("--cx", type=int, default=1_000_000_000)
     ap.add_argument("--cs", type=int, default=255)
@@ -455,6 +569,15 @@ def main(argv=None):
     if len(a.inputs) < 2:
         ap.error("give at least one input and the output prefix")
     parse = "gpu" if a.gpu_parse else "host"
+    if a.e:
+        if a.b:
+            ap.error("k-mer histogram estimation possible only for canonical k-mers")
+        if not 1 <= a.k <= ESTIMATE_MAX_K:
+            ap.error("-e takes k = 1..%d" % ESTIMATE_MAX_K)
+        write_histogram(a.inputs[-1], estimate_histogram(a.inputs[:-1], a.k, None, a.batch_bytes, a.device, parse))
+        return 0
+    if a.opt_out_size and a.lut_prefix_len is not None:
+        ap.error("--opt-out-size picks the LUT prefix length: it cannot be combined with --lut-prefix-len")
     if a.map_from:
         m, sig_map = signature_map_from_kmc_pre(a.map_from)
     elif a.map:
@@ -462,13 +585,15 @@ def main(argv=None):
     else:
         m, sig_map = a.signature_len, None
     if a.small_k or a.k <= m:                                           # no bins: no map, and the path picks its own LUT prefix length
+        if a.opt_out_size:
+            ap.error("histogram estimation is not supported on the small-k path, as in kmc")
         print(json.dumps(count_reads_small_k(a.inputs[:-1], a.inputs[-1], a.k, a.ci, a.cx, a.cs, not a.b, a.batch_bytes, a.device, parse)))
         return 0
     lp = a.lut_prefix_len
-    if lp is None:
+    if lp is None and not a.opt_out_size:
         lp = next(p for p in (7, 3, 11, 15, 4, 5, 6, 2, 8, 9, 10, 12, 13, 14, 1) if p < a.k and (a.k - p) % 4 == 0)
     res = count_reads(a.inputs[:-1], a.inputs[-1], a.k, m, sig_map, lp, a.ci, a.cx, a.cs, not a.b, a.batch_bytes, a.device,
-                      a.n_bins if sig_map is None else None, parse=parse, small_k=False)
+                      a.n_bins if sig_map is None else None, parse=parse, small_k=False, opt_out_size=a.opt_out_size)
     print(json.dumps(res))
     return 0
 

@@ -445,6 +445,10 @@ int kmcb200_stage_times(kmcb200_ctx* ctx, uint32_t slot, float* ms, uint32_t cap
 /* Comma-separated names of the timed sort intervals ms[3..] of kmcb200_stage_times ("msd_partition_L1,msd_count_L2,...").
  * Returns their number. */
 int kmcb200_stage_names(kmcb200_ctx* ctx, uint32_t slot, char* buf, uint32_t capacity);
+/* How the last bin of a slot counted its leaves: out[0] = the bits of the second partition level, out[1] = the leaf kernel
+ * (KMCB200_LEAF_*; KMCB200_LEAF_NONE when the bin's leaves were sorted, e.g. a bin too small for the MSD path).  Returns 0, negative on error. */
+enum { KMCB200_LEAF_NONE = 0, KMCB200_LEAF_HASH = 1, KMCB200_LEAF_HASH_CTA = 2, KMCB200_LEAF_HASH_WIDE = 3 };
+int kmcb200_leaf_plan(kmcb200_ctx* ctx, uint32_t slot, uint32_t* out);
 
 #ifdef __cplusplus
 }

@@ -65,7 +65,7 @@ EXPORTS = [
     "kmcb200_create", "kmcb200_destroy", "kmcb200_last_error", "kmcb200_out_rec_bytes", "kmcb200_out_capacity", "kmcb200_lut_entries",
     "kmcb200_host_alloc", "kmcb200_host_free", "kmcb200_process_bin", "kmcb200_process_bin_multi", "kmcb200_submit_bin", "kmcb200_submit_bin_indexed", "kmcb200_wait_bin", "kmcb200_sort_records",
     "kmcb200_dev_process_bin", "kmcb200_dev_expand", "kmcb200_dev_sort", "kmcb200_dev_count", "kmcb200_kernel_launches",
-    "kmcb200_stage_times", "kmcb200_stage_names",
+    "kmcb200_stage_times", "kmcb200_stage_names", "kmcb200_leaf_plan",
     "kmcb200_wait_bin_scanned", "kmcb200_db_open", "kmcb200_db_last_error", "kmcb200_db_records", "kmcb200_db_reserve", "kmcb200_db_commit_bin", "kmcb200_db_close",
     "kmcb200_splitter_create", "kmcb200_splitter_destroy", "kmcb200_splitter_last_error", "kmcb200_split", "kmcb200_dev_split",
     "kmcb200_splitter_kernel_launches", "kmcb200_splitter_count_kxmers", "kmcb200_splitter_kxmer_totals",
@@ -125,6 +125,7 @@ def load_library(build_if_needed=True):
     L.kmcb200_kernel_launches.restype = u64
     L.kmcb200_stage_times.argtypes = [vp, u32, C.POINTER(C.c_float), u32]
     L.kmcb200_stage_names.argtypes = [vp, u32, C.c_char_p, u32]
+    L.kmcb200_leaf_plan.argtypes = [vp, u32, C.POINTER(C.c_uint32)]
     L.kmcb200_wait_bin_scanned.argtypes = [vp, u32, u64, C.POINTER(u64), vp]
     L.kmcb200_db_open.argtypes = [C.POINTER(_DbParams), C.c_char_p, u64, C.POINTER(vp)]
     L.kmcb200_db_last_error.argtypes = [vp]
@@ -303,6 +304,15 @@ class Stage2Context(_Handle):
         self._check(self.lib.kmcb200_stage_names(self._h, slot, names, 2048))
         nm = names.value.decode().split(",") if names.value else []
         return {"expand_ms": ms[0], "sort_ms": ms[1], "count_ms": ms[2], "pass_ms": [ms[3 + i] for i in range(n)], "pass_names": nm}
+
+    LEAF_KERNELS = {0: None, 1: "hash", 2: "cta", 3: "wide"}
+
+    def leaf_plan(self, slot=0):
+        """How the slot's last bin counted its leaves: (bits of the second partition level, leaf kernel: "hash" = leaf_hash_kernel,
+        "cta" = leaf_hash_cta_kernel, "wide" = leaf_hash_wide_kernel, None = the leaves were sorted)."""
+        out = (C.c_uint32 * 2)()
+        self._check(self.lib.kmcb200_leaf_plan(self._h, slot, out))
+        return int(out[0]), self.LEAF_KERNELS[int(out[1])]
 
     # -- seam #2, host buffers
     def process_bin(self, b: SuperKmerBin, out=None, lut=None, bin_id=0) -> BinResult:

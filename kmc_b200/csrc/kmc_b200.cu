@@ -109,6 +109,7 @@ struct Slot {
 	cudaEvent_t ev_h2d = nullptr, ev_done = nullptr, ev_walk = nullptr;           // copy stream <-> compute stream hand-over
 	cudaEvent_t ev_pass[kMaxPasses + 8] = {};
 	int n_passes_run = 0;                                   // number of timed sort intervals (ev_pass[i] .. ev_pass[i+1])
+	uint32_t leaf_b2 = 0, leaf_kernel = 0;                  // counted leaves of the last bin: level-2 bits, kernel (kmcb200_leaf_plan; 0: not counted)
 	bool ran_expand = false, ran_sort = false, ran_count = false;
 	// oversized bins
 	DevBuf<uint64_t> d_hist12; DevBuf<unsigned long long> d_out_counter;
@@ -259,11 +260,18 @@ __global__ void msd_setup_kernel(uint64_t* seg1, uint32_t* item_base1, uint32_t*
 	*n_items1 = nt;
 }
 
-// bits of the second partition level.  Counted leaves (the bin path) are streamed by one warp and may be any size: a leaf beyond one
-// table round only costs extra rounds, while the 512 / 1024-digit partition kernels are slower per record than the 256-digit one.
+// One-word bins take 7 level-2 bits, not 8, while their mean leaf at 7 bits is at most this many records.  leaf_hash_cta_kernel counts
+// ~8 K records of a 30x bin in one table round and the leaves spread over 0 .. 2x their mean, so up to here few leaves need a second
+// round, and the 128-digit count and partition are cheaper than the 256-digit ones (DESIGN 3.1, H100: a bin of 1.01x10^8 k-mers 7 %
+// faster, 2^27 5 %, 1.68x10^8 about even; at 2.01x10^8 the 6 K-record mean leaves need second rounds and 8 bits win).
+constexpr uint64_t kL2SevenBitsMaxMean = 5120;
+
+// bits of the second partition level.  Counted leaves (the bin path) are streamed by one warp or CTA and may be any size: a leaf beyond
+// one table round only costs extra rounds, while the 512 / 1024-digit partition kernels are slower per record than the 256-digit one.
 // So: leaves of ~1 K records, in at most 8 bits for one-word records (DESIGN 3.1: on the H100 the wider level 2 costs more than it saves
-// at every bin size of the target workload) and at most 10 bits for wider ones (their leaves verify every hit against a record in HBM and
-// lose more from a second table round than the wide scatter costs).
+// at every bin size of the target workload) - and in at most 7 while that leaves a mean leaf of kL2SevenBitsMaxMean records or fewer,
+// which the CTA kernel counts - and at most 10 bits for wider ones (their leaves verify every hit against a record in HBM and lose more
+// from a second table round than the wide scatter costs).
 // Sorted leaves (seam #1) must fit on chip, and canonical k-mers crowd into the low prefixes (largest leaf ~4.4x the mean): aim at a
 // fifth of the capacity, 8 bits at most.
 template <int WORDS>
@@ -272,7 +280,7 @@ uint32_t choose_b2(const kmcb200_ctx* ctx, uint64_t n, bool counted_leaves)
 	auto bits_for = [&](uint64_t target) { uint32_t lg = 0; while ((1ull << lg) < (n + target - 1) / target) ++lg; return lg > 8 ? lg - 8 : 0u; };
 	uint32_t b2;
 	if (counted_leaves) {
-		b2 = std::min(bits_for(1024), WORDS == 1 ? 8u : 10u);
+		b2 = std::min(bits_for(1024), WORDS == 1 ? (n <= (kL2SevenBitsMaxMean << 15) ? 7u : 8u) : 10u);
 		if (ctx->force_b2) b2 = ctx->force_b2;          // (tests: the wide second level on small bins)
 	} else
 		b2 = std::min(bits_for(std::max<uint64_t>(msd_local_cap<WORDS>() / 5, 64)), 8u);
@@ -688,8 +696,8 @@ int setup_leaf_cta(kmcb200_ctx* ctx)
 
 // leaf_hash_cta_kernel takes the bins whose mean leaf (records / leaves) is larger than this.  Its gain is that a leaf of up to ~8 K records
 // of a 30x bin is one table round where a warp's table needs 2 .. 4 (leaves spread over 0 .. 2x their mean; a warp's round holds ~1800
-// records); for leaves that already fit one warp round, the warp kernel's independent warps are faster (DESIGN 3.2: 0.58 against
-// 0.77 ms for a 2^26-k-mer bin, mean leaf 1024, on an H100).
+// records); for leaves that already fit one warp round, the warp kernel's independent warps are faster (DESIGN 3.2, H100: a 2^25-k-mer
+// bin in 7 bits, mean leaf 1024, 0.31 against 0.40 ms; a 2^26-k-mer bin in 7 bits, mean leaf 2048, 0.78 against 0.62 ms).
 constexpr uint64_t kLeafCtaMinMean = 1280;
 
 constexpr int kLeafSlotBits = 10;          // a warp's leaf table (leaf_hash_kernel, leaf_hash_wide_kernel, leaf_warp_kernel): 2^10 slots
@@ -697,7 +705,7 @@ constexpr int kLeafSlotBits = 10;          // a warp's leaf table (leaf_hash_ker
 #define DISPATCH_CTA(ctx, fn, ...) ((ctx)->leaf_cta_slot_bits == 10 ? fn<4, 10>(__VA_ARGS__) : fn<4, 12>(__VA_ARGS__))
 
 template <int WORDS>
-int launch_leaves(kmcb200_ctx* ctx, const LeafArgs& la, uint64_t n_rec, cudaStream_t st)
+int launch_leaves(kmcb200_ctx* ctx, const LeafArgs& la, uint64_t n_rec, cudaStream_t st, uint32_t* kernel)
 {
 	const size_t hsmem = sizeof(LhSmem<kLeafSlotBits>) * kLwWarps;
 	const uint32_t hgrid = std::min<uint32_t>((la.n_leaves + kLwWarps - 1) / kLwWarps, (uint32_t)(ctx->sm_count * ctx->occ_leaf_hash));
@@ -705,10 +713,12 @@ int launch_leaves(kmcb200_ctx* ctx, const LeafArgs& la, uint64_t n_rec, cudaStre
 	const uint32_t max_count = WORDS == 1 ? kLwHeavy : kLwMaxLeaf;
 	const bool simple = la.cutoff_min >= 2u && la.cutoff_max >= la.cutoff_min && (la.cutoff_max + 1u == 0u || la.cutoff_max + 1u > max_count + 1u);
 	if constexpr (WORDS == 1) {
-		if (ctx->leaf_cta == 1 || (ctx->leaf_cta == 2 && n_rec > kLeafCtaMinMean * la.n_leaves)) DISPATCH_CTA(ctx, launch_leaf_cta, ctx, la, simple, st);
+		*kernel = ctx->leaf_cta == 1 || (ctx->leaf_cta == 2 && n_rec > kLeafCtaMinMean * la.n_leaves) ? KMCB200_LEAF_HASH_CTA : KMCB200_LEAF_HASH;
+		if (*kernel == KMCB200_LEAF_HASH_CTA) DISPATCH_CTA(ctx, launch_leaf_cta, ctx, la, simple, st);
 		else if (simple) leaf_hash_kernel<kLeafSlotBits, true><<<hgrid, 32 * kLwWarps, hsmem, st>>>(la);
 		else leaf_hash_kernel<kLeafSlotBits, false><<<hgrid, 32 * kLwWarps, hsmem, st>>>(la);
 	} else {
+		*kernel = KMCB200_LEAF_HASH_WIDE;
 		if (simple) leaf_hash_wide_kernel<WORDS, kLeafSlotBits, true><<<hgrid, 32 * kLwWarps, hsmem, st>>>(la);
 		else leaf_hash_wide_kernel<WORDS, kLeafSlotBits, false><<<hgrid, 32 * kLwWarps, hsmem, st>>>(la);
 	}
@@ -767,6 +777,7 @@ int run_sort_count_leaves(kmcb200_ctx* ctx, Slot& s, uint64_t n_rec, uint32_t np
 	// the sort starts below those bits, and nobody has counted the first digit yet
 	bool in_b = false;
 	LeafPlan plan;
+	s.leaf_b2 = 0; s.leaf_kernel = 0;
 	if (int rc = launch_sort<WORDS>(ctx, s, ra, rb, n_rec, ctx->key_bytes, 2u * ctx->prm.kmer_len - block_bits, from_blocks ? (int)kHistNone : s.hist_mode, np_eff, st, &in_b, &plan)) return rc;
 	if (!plan.active) {          // small bin: plain LSD passes, classic count
 		CU(ctx, cudaEventRecord(s.ev_sort, st));
@@ -790,7 +801,8 @@ int run_sort_count_leaves(kmcb200_ctx* ctx, Slot& s, uint64_t n_rec, uint32_t np
 	la.counter_max = ctx->prm.counter_max; la.counter_bytes = ctx->counter_bytes; la.suffix_bytes = ctx->suffix_bytes;
 	la.heavy_list = s.zero->heavy_list; la.heavy_count = &s.zero->heavy_count[0]; la.heavy_ticket = &s.zero->heavy_count[1]; la.heavy_cap = kHeavyListCap;
 	la.tmp = s.leaf_tmp; la.leaf_emit = s.leaf_emit; la.group_sum = s.zero->leaf_group_sum; la.lut = d_lut; la.result = d_result; la.ticket = &s.zero->msd_counters[3]; la.flags = flags;
-	if (int rc = launch_leaves<WORDS>(ctx, la, n_rec, st)) return rc;
+	s.leaf_b2 = 31 - __builtin_clz(plan.n_leaves) - 8;          // (n_leaves = 256 << b2)
+	if (int rc = launch_leaves<WORDS>(ctx, la, n_rec, st, &s.leaf_kernel)) return rc;
 	if constexpr (WORDS == 1) {          // the large leaves the main launch only noted (none in a typical bin: the launch returns at once)
 		if (int rc = launch_heavy_leaves(ctx, la, st)) return rc;
 	}
@@ -1653,6 +1665,15 @@ int kmcb200_stage_names(kmcb200_ctx* ctx, uint32_t slot, char* buf, uint32_t cap
 	for (int p = 0; p < s.n_passes_run; ++p) { if (p) out += ","; out += s.pass_names[p] ? s.pass_names[p] : "?"; }
 	snprintf(buf, capacity, "%s", out.c_str());
 	return s.n_passes_run;
+}
+
+int kmcb200_leaf_plan(kmcb200_ctx* ctx, uint32_t slot, uint32_t* out)
+{
+	if (int rc = check_slot(ctx, slot)) return rc;
+	if (!out) return fail(ctx, KMCB200_ERR_INVALID, "out");
+	const Slot& s = ctx->slots[slot];
+	out[0] = s.leaf_b2; out[1] = s.leaf_kernel;
+	return 0;
 }
 
 }  // extern "C"

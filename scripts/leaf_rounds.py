@@ -23,7 +23,7 @@ def b2_for(n):
     lg = 0
     while (1 << lg) < (n + 1023) // 1024:
         lg += 1
-    return min(max(lg - 8, 0), 8)
+    return min(max(lg - 8, 0), 7 if n <= 5120 << 15 else 8)          # (kL2SevenBitsMaxMean)
 
 
 def reads_per_record(sizes, distinct, ratio, slots):

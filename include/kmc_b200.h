@@ -214,6 +214,17 @@ int kmcb200_splitter_count_kxmers(kmcb200_splitter* sp, int both_strands);
 /* per_bin[n_bins]: the totals since kmcb200_splitter_count_kxmers (waits for the device's queued work).  KMCB200_ERR_INVALID when the
  * counting was never enabled. */
 int kmcb200_splitter_kxmer_totals(kmcb200_splitter* sp, uint64_t* per_bin);
+/* Homopolymer compression (`kmc -hc`, CSplitter::HomopolymerCompressSeq, splitter.cpp:424-435), opt-in, on (1) or off (0) for the calls
+ * that follow.  While it is on, every batch entry point of the handle (the host batch, the device twin, the raw-chunk form after its
+ * parse) first compresses the batch on the device: a byte of ACGTacgt that repeats the base before it, ignoring case, is dropped, and the
+ * result is padded back to the batch's length with '\n' (no k-mer, record or count comes from a separator).  Runs never cross a
+ * separator, so each read is compressed on its own, as in the reference; the caller's batch is read and never written, and *consumed /
+ * *seq_bytes keep their meaning (the parsed batch).  Work: 3 more kernel launches per call with a non-empty batch, no host
+ * synchronisation.  Workspace: 1 B per byte of max_batch_bytes plus 8 B per 16 KiB, allocated the first time compression is turned on
+ * and kept until the handle is destroyed; a handle that never turns it on allocates, launches and writes exactly as without this call.
+ * The same call exists for the signature statistics and the small-k counter.  The histogram estimator has none: the reference never
+ * compresses the reads it estimates from (`kmc -e -hc` writes the file `kmc -e` writes). */
+int kmcb200_splitter_set_homopolymer_compressed(kmcb200_splitter* sp, int on);
 
 /* ---- stage 0: signature statistics (CKMC::buildSignatureMapping, kmc_core/kmc.h:974-1075) ----------------------------------------
  * Before it splits, the reference counts the k-mers of every signature over a sample of the input (CSplitter::CalcStats,
@@ -252,6 +263,9 @@ int kmcb200_sigstats_read(kmcb200_sigstats* h, uint32_t* counts);
 int kmcb200_sigstats_reset(kmcb200_sigstats* h);
 /* Number of kernels this handle has launched so far. */
 uint64_t kmcb200_sigstats_kernel_launches(const kmcb200_sigstats* h);
+/* Homopolymer compression before the statistics, as kmcb200_splitter_set_homopolymer_compressed describes (CSplitter::CalcStats,
+ * splitter.cpp:457-458): 3 more launches per non-empty batch. */
+int kmcb200_sigstats_set_homopolymer_compressed(kmcb200_sigstats* h, int on);
 /* map[4^signature_len + 1].  KMCB200_ERR_INVALID: signature_len outside 5..11, n_bins outside 2..KMCB200_SPLIT_MAX_BINS (one bin besides
  * the special signature's is needed), or counts for which the rule would hand out an id >= n_bins. */
 int kmcb200_signature_map(const uint32_t* counts, uint32_t signature_len, uint32_t n_bins, int32_t* map);
@@ -341,6 +355,9 @@ void kmcb200_smallk_destroy(kmcb200_smallk* h);
 const char* kmcb200_smallk_last_error(const kmcb200_smallk* h);
 /* Number of kernels this handle has launched so far. */
 uint64_t kmcb200_smallk_kernel_launches(const kmcb200_smallk* h);
+/* Homopolymer compression before the count, as kmcb200_splitter_set_homopolymer_compressed describes (CSplitter::ProcessReadsSmallK,
+ * splitter.cpp:702-703, 757-758): 3 more launches per non-empty batch. */
+int kmcb200_smallk_set_homopolymer_compressed(kmcb200_smallk* h, int on);
 /* Host batch: copied in, counted; returns when the batch buffer may be reused.  A batch over max_batch_bytes: KMCB200_ERR_INVALID. */
 int kmcb200_smallk_add(kmcb200_smallk* h, const uint8_t* seq, uint64_t bytes);
 /* Device twin: d_seq in HBM, queued on `stream` (a cudaStream_t; NULL = the legacy default stream) after the handle's earlier work. */

@@ -69,6 +69,7 @@ EXPORTS = [
     "kmcb200_wait_bin_scanned", "kmcb200_db_open", "kmcb200_db_last_error", "kmcb200_db_records", "kmcb200_db_reserve", "kmcb200_db_commit_bin", "kmcb200_db_close",
     "kmcb200_splitter_create", "kmcb200_splitter_destroy", "kmcb200_splitter_last_error", "kmcb200_split", "kmcb200_dev_split",
     "kmcb200_splitter_kernel_launches", "kmcb200_splitter_count_kxmers", "kmcb200_splitter_kxmer_totals",
+    "kmcb200_splitter_set_homopolymer_compressed", "kmcb200_sigstats_set_homopolymer_compressed", "kmcb200_smallk_set_homopolymer_compressed",
     "kmcb200_sigstats_create", "kmcb200_sigstats_destroy", "kmcb200_sigstats_last_error", "kmcb200_sigstats_add", "kmcb200_dev_sigstats_add",
     "kmcb200_sigstats_read", "kmcb200_sigstats_reset", "kmcb200_sigstats_kernel_launches", "kmcb200_signature_map", "kmcb200_stage2_bin_order",
     "kmcb200_fastx_create", "kmcb200_fastx_destroy", "kmcb200_fastx_last_error", "kmcb200_fastx_kernel_launches", "kmcb200_fastx_parse",
@@ -146,6 +147,9 @@ def load_library(build_if_needed=True):
     L.kmcb200_splitter_kernel_launches.restype = u64
     L.kmcb200_splitter_count_kxmers.argtypes = [vp, C.c_int]
     L.kmcb200_splitter_kxmer_totals.argtypes = [vp, vp]
+    L.kmcb200_splitter_set_homopolymer_compressed.argtypes = [vp, C.c_int]
+    L.kmcb200_sigstats_set_homopolymer_compressed.argtypes = [vp, C.c_int]
+    L.kmcb200_smallk_set_homopolymer_compressed.argtypes = [vp, C.c_int]
     L.kmcb200_sigstats_create.argtypes = [C.POINTER(_SigstatsParams), C.POINTER(vp)]
     L.kmcb200_sigstats_destroy.argtypes = [vp]
     L.kmcb200_sigstats_destroy.restype = None
@@ -436,10 +440,11 @@ class Splitter(_Handle):
     """Stage 1 on one GPU (kmcb200_splitter_*): batches of sequences -> KMC bins (CSplitter::ProcessReads, kmc_core/splitter.cpp:557-677).
 
     A batch is one byte array in which every byte other than ACGTacgt separates (reads.sequences_to_batch makes one from FASTQ / FASTA).
-    `signature_map` has 4^signature_len + 1 entries, each below n_bins."""
+    `signature_map` has 4^signature_len + 1 entries, each below n_bins.  homopolymer_compressed: every batch is homopolymer-compressed on
+    the GPU first, as `kmc -hc` does (see set_homopolymer_compressed)."""
     _prefix = "kmcb200_splitter"
 
-    def __init__(self, kmer_len, signature_len, signature_map, n_bins=None, device=0, max_batch_bytes=1 << 26):
+    def __init__(self, kmer_len, signature_len, signature_map, n_bins=None, device=0, max_batch_bytes=1 << 26, homopolymer_compressed=False):
         sig_map = np.ascontiguousarray(signature_map, dtype=np.uint32)
         if sig_map.size != (1 << (2 * signature_len)) + 1:
             raise KmcB200Error(ERR_INVALID, "signature_map has %d entries, 4^%d + 1 expected" % (sig_map.size, signature_len))
@@ -449,6 +454,8 @@ class Splitter(_Handle):
         self._open(C.byref(p), sig_map.ctypes.data)
         self._out = np.empty(0, dtype=np.uint8)
         self._packs = np.empty(0, dtype=np.uint64)
+        if homopolymer_compressed:
+            self.set_homopolymer_compressed(True)
 
     def kernel_launches(self):
         return int(self.lib.kmcb200_splitter_kernel_launches(self._h))
@@ -508,6 +515,12 @@ class Splitter(_Handle):
         """From now on every split also counts, per bin, the collector's (k+x)-mers (n_plus_x_recs); zeroes the totals."""
         self._check(self.lib.kmcb200_splitter_count_kxmers(self._h, int(bool(both_strands))))
 
+    def set_homopolymer_compressed(self, on=True):
+        """kmcb200_splitter_set_homopolymer_compressed: while on, every batch (host, device twin or parsed chunk) has each run of one base
+        collapsed to a single base on the GPU before it is split, as `kmc -hc` does; 3 more kernel launches per batch and
+        max_batch_bytes more bytes of HBM, allocated the first time it is turned on."""
+        self._check(self.lib.kmcb200_splitter_set_homopolymer_compressed(self._h, int(bool(on))))
+
     def kxmer_totals(self):
         """uint64[n_bins]: the (k+x)-mers per bin since count_kxmers (zeros for k % 32 == 0, where stage 2 sorts plain k-mers)."""
         out = np.zeros(self.n_bins, dtype=np.uint64)
@@ -517,13 +530,22 @@ class Splitter(_Handle):
 
 class SignatureStats(_Handle):
     """Stage 0 on one GPU (kmcb200_sigstats_*): k-mers per signature over batches of sequences, what CSplitter::CalcStats counts
-    (kmc_core/splitter.cpp:439-533).  Batches as for Splitter; the counts (uint32[4^signature_len + 1]) add up until reset()."""
+    (kmc_core/splitter.cpp:439-533).  Batches as for Splitter; the counts (uint32[4^signature_len + 1]) add up until reset().
+    homopolymer_compressed as for Splitter."""
     _prefix = "kmcb200_sigstats"
 
-    def __init__(self, kmer_len, signature_len, device=0, max_batch_bytes=1 << 26):
+    def __init__(self, kmer_len, signature_len, device=0, max_batch_bytes=1 << 26, homopolymer_compressed=False):
         self.kmer_len, self.signature_len, self.max_batch_bytes = kmer_len, signature_len, max_batch_bytes
         p = _SigstatsParams(kmer_len, signature_len, device, 0, max_batch_bytes)
         self._open(C.byref(p))
+        if homopolymer_compressed:
+            self.set_homopolymer_compressed(True)
+
+    def set_homopolymer_compressed(self, on=True):
+        """kmcb200_sigstats_set_homopolymer_compressed: while on, every batch (host, device twin or parsed chunk) has each run of one base
+        collapsed to a single base on the GPU before it is counted, as `kmc -hc` does; 3 more kernel launches per batch and
+        max_batch_bytes more bytes of HBM, allocated the first time it is turned on."""
+        self._check(self.lib.kmcb200_sigstats_set_homopolymer_compressed(self._h, int(bool(on))))
 
     def kernel_launches(self):
         return int(self.lib.kmcb200_sigstats_kernel_launches(self._h))
@@ -558,13 +580,21 @@ class SmallKCounter(_Handle):
     """Small k (1..13) on one GPU (kmcb200_smallk_*), KMC's small-k mode (kmc_core/kmc.h:677-960): every k-mer of the batches counted in
     a direct array of 4^k uint64 counters (CSplitter::ProcessReadsSmallK), then a KMC1-format database (CSmallKCompleter).  Batches as for
     Splitter; the counts add up until reset().  There are no bins, so no signature length, map or caller-chosen LUT prefix length: finish()
-    picks the LUT prefix length as the reference does."""
+    picks the LUT prefix length as the reference does.  homopolymer_compressed as for Splitter."""
     _prefix = "kmcb200_smallk"
 
-    def __init__(self, kmer_len, both_strands=True, device=0, max_batch_bytes=1 << 26):
+    def __init__(self, kmer_len, both_strands=True, device=0, max_batch_bytes=1 << 26, homopolymer_compressed=False):
         self.kmer_len, self.both_strands, self.max_batch_bytes = kmer_len, bool(both_strands), max_batch_bytes
         p = _SmallKParams(kmer_len, int(bool(both_strands)), device, 0, max_batch_bytes)
         self._open(C.byref(p))
+        if homopolymer_compressed:
+            self.set_homopolymer_compressed(True)
+
+    def set_homopolymer_compressed(self, on=True):
+        """kmcb200_smallk_set_homopolymer_compressed: while on, every batch (host, device twin or parsed chunk) has each run of one base
+        collapsed to a single base on the GPU before it is counted, as `kmc -hc` does; 3 more kernel launches per batch and
+        max_batch_bytes more bytes of HBM, allocated the first time it is turned on."""
+        self._check(self.lib.kmcb200_smallk_set_homopolymer_compressed(self._h, int(bool(on))))
 
     def kernel_launches(self):
         return int(self.lib.kmcb200_smallk_kernel_launches(self._h))

@@ -15,6 +15,7 @@
 #include "leaf_hash_wide.cuh"
 #include "split.cuh"
 #include "fastx.cuh"
+#include "hc.cuh"
 #include "small_k.cuh"
 #include "estimate.cuh"
 
@@ -1679,6 +1680,7 @@ int kmcb200_leaf_plan(kmcb200_ctx* ctx, uint32_t slot, uint32_t* out)
 }  // extern "C"
 
 #include "db_writer.inl"
+#include "hc.inl"
 #include "splitter.inl"
 #include "stage0.inl"
 #include "fastx.inl"

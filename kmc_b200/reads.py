@@ -31,6 +31,15 @@ Histogram estimation (`estimate_histogram`, `-e`): KMC's ntHash estimator (`kmc 
 the chunks it splits and picks the LUT prefix length from the estimated number of counted k-mers, as `kmc --opt-out-size` does.
 
     python -m kmc_b200.reads -e -k31 reads.fq hist.txt
+
+Homopolymer compression (`homopolymer_compressed=True`, `--hc`): `kmc -hc`.  Every run of one base in a read (case ignored) is collapsed
+to a single base on the GPU before the statistics, the split and the small-k count see it (Splitter / SignatureStats / SmallKCounter
+set_homopolymer_compressed).  The histogram estimator sees the reads uncompressed, as in the reference, so `-e --hc` writes the file `-e`
+writes and `--opt-out-size --hc` picks the LUT prefix length from the uncompressed k-mers.  n_bases counts the input bases; n_kmers and
+n_super_kmers are counted after compression.  The files are `kmc -hc -sr1`'s for records shorter than 524,296 symbols: the reference cuts
+longer records into parts and compresses each part on its own (DESIGN.md section 3.13), the GPU compresses every record whole.
+
+    python -m kmc_b200.reads --hc -k31 reads.fq out_prefix
 """
 import argparse
 import json
@@ -234,12 +243,13 @@ class _Parsers:
         self.by_format = {}
 
 
-def signature_sample_counts(paths, k, signature_len, batch_bytes=1 << 26, device=0, parse="host"):
+def signature_sample_counts(paths, k, signature_len, batch_bytes=1 << 26, device=0, parse="host", homopolymer_compressed=False):
     """Stage 0's statistics (CKMC::buildSignatureMapping, kmc_core/kmc.h:974-1075): k-mers per signature, counted on the GPU, over the
     raw bytes of the files in input order up to the end of the first record at or beyond max(2^28, total bytes / 100).
-    parse="gpu": the files are parsed on the GPU in chunks of batch_bytes - 1, the sample's end found by the parser's limit."""
+    parse="gpu": the files are parsed on the GPU in chunks of batch_bytes - 1, the sample's end found by the parser's limit.
+    homopolymer_compressed: the k-mers of the compressed reads are counted (`kmc -hc`); the sample's end is still found on the raw bytes."""
     budget = max(STATS_SAMPLE_BYTES, sum(os.path.getsize(p) for p in paths) // 100)
-    st = SignatureStats(k, signature_len, device, max_batch_bytes=batch_bytes)
+    st = SignatureStats(k, signature_len, device, max_batch_bytes=batch_bytes, homopolymer_compressed=homopolymer_compressed)
     if parse == "gpu":
         parsers = _Parsers(device, batch_bytes - 1)
         try:
@@ -364,17 +374,18 @@ def write_histogram(path, hist):
 
 
 def count_reads_small_k(paths, out_prefix, k, cutoff_min=2, cutoff_max=1_000_000_000, counter_max=255, both_strands=True, batch_bytes=1 << 26,
-                        device=0, parse="host"):
+                        device=0, parse="host", homopolymer_compressed=False):
     """KMC's small-k mode (kmc_core/kmc.h:677-960) on one GPU, for 1 <= k <= 13: every batch of every file is counted into 4^k counters
     (kmc_b200.SmallKCounter), then the KMC1 database is written (CSmallKCompleter::CompleteKMCFormat).  There are no bins: no signature
     length, no map, and the LUT prefix length is the reference's choice for this mode, returned as `lut_prefix_len`.  parse as for
-    count_reads.  Returns the keys count_reads returns (n_super_kmers is 0, n_kmers equals n_total) plus lut_prefix_len."""
+    count_reads.  homopolymer_compressed: `kmc -hc` (see the module docstring).  Returns the keys count_reads returns (n_super_kmers is 0,
+    n_kmers equals n_total) plus lut_prefix_len."""
     if parse not in ("host", "gpu"):
         raise KmcB200Error(ERR_INVALID, "parse must be 'host' or 'gpu', not %r" % (parse,))
     if not 1 <= k <= SMALL_K_MAX:
         raise KmcB200Error(ERR_INVALID, "the small-k path counts k = 1..%d, not %d" % (SMALL_K_MAX, k))
     t0 = time.perf_counter()
-    sk = SmallKCounter(k, both_strands, device, max_batch_bytes=batch_bytes)
+    sk = SmallKCounter(k, both_strands, device, max_batch_bytes=batch_bytes, homopolymer_compressed=homopolymer_compressed)
     n_bases = 0
     read_s = 0.0
     parsers = _Parsers(device, batch_bytes - 1) if parse == "gpu" else None
@@ -412,7 +423,8 @@ def count_reads_small_k(paths, out_prefix, k, cutoff_min=2, cutoff_max=1_000_000
 
 
 def count_reads(paths, out_prefix, k, signature_len, signature_map, lut_prefix_len=None, cutoff_min=2, cutoff_max=1_000_000_000, counter_max=255,
-                both_strands=True, batch_bytes=1 << 26, device=0, n_bins=None, parse="host", small_k=None, opt_out_size=False):
+                both_strands=True, batch_bytes=1 << 26, device=0, n_bins=None, parse="host", small_k=None, opt_out_size=False,
+                homopolymer_compressed=False):
     """KMC's stages on one GPU in RAM mode: every batch of every file is split on the GPU and the bin fragments stay in host memory;
     then bin by bin, stage 2 and the database writer.  Returns the writer's totals and the split's counts.
     With a signature_map: the bins are written in bin-id order, bin b's signatures (the map's preimage of b) go into .kmc_pre, and n_bins
@@ -428,7 +440,9 @@ def count_reads(paths, out_prefix, k, signature_len, signature_map, lut_prefix_l
     lut_prefix_len=None picks it as `kmc` does (kmc_lut_prefix_len): from 4 * n_reads, the records of the input (FASTQ records, FASTA
     headers), or with opt_out_size=True from the estimate of the counted k-mers, which the histogram estimator (HistogramEstimator, s by
     estimate_s) computes over the same batches as the split, as `kmc --opt-out-size` does.  opt_out_size needs canonical k-mers and the
-    bin path.  The result holds n_reads and the lut_prefix_len used."""
+    bin path.  The result holds n_reads and the lut_prefix_len used.
+    homopolymer_compressed=True counts the k-mers of the homopolymer-compressed reads, as `kmc -hc` does: stage 0, the split and the
+    small-k path compress every batch on the GPU; the estimator and n_reads see the reads as they are (see the module docstring)."""
     if parse not in ("host", "gpu"):
         raise KmcB200Error(ERR_INVALID, "parse must be 'host' or 'gpu', not %r" % (parse,))
     if opt_out_size and not both_strands:
@@ -438,11 +452,13 @@ def count_reads(paths, out_prefix, k, signature_len, signature_map, lut_prefix_l
     if small_k or (small_k is None and k <= signature_len):
         if opt_out_size:
             raise KmcB200Error(ERR_INVALID, "histogram estimation is not supported on the small-k path, as in kmc")
-        return count_reads_small_k(paths, out_prefix, k, cutoff_min, cutoff_max, counter_max, both_strands, batch_bytes, device, parse)
+        return count_reads_small_k(paths, out_prefix, k, cutoff_min, cutoff_max, counter_max, both_strands, batch_bytes, device, parse,
+                                   homopolymer_compressed)
     t0 = time.perf_counter()
     if signature_map is None:
         n_bins = DEFAULT_N_BINS if n_bins is None else int(n_bins)
-        mapper = _signature_map(signature_sample_counts(paths, k, signature_len, batch_bytes, device, parse), signature_len, n_bins)
+        mapper = _signature_map(signature_sample_counts(paths, k, signature_len, batch_bytes, device, parse, homopolymer_compressed),
+                                signature_len, n_bins)
         sig_map = np.maximum(mapper, 0).astype(np.uint32)              # no k-mer has a signature that is not allowed
     else:
         mapper = None
@@ -450,7 +466,7 @@ def count_reads(paths, out_prefix, k, signature_len, signature_map, lut_prefix_l
         n_bins = int(sig_map.max()) + 1 if n_bins is None else int(n_bins)
     t_stats = time.perf_counter() - t0
     # the splitter first: the stage-2 context sizes its block limit from the HBM that is free when it is created
-    sp = Splitter(k, signature_len, sig_map, n_bins, device, max_batch_bytes=batch_bytes)
+    sp = Splitter(k, signature_len, sig_map, n_bins, device, max_batch_bytes=batch_bytes, homopolymer_compressed=homopolymer_compressed)
     if mapper is not None:
         sp.count_kxmers(both_strands)
     est = HistogramEstimator(k, estimate_s(paths), device, max_batch_bytes=batch_bytes) if opt_out_size else None
@@ -560,6 +576,7 @@ def main(argv=None):
     ap.add_argument("--cx", type=int, default=1_000_000_000)
     ap.add_argument("--cs", type=int, default=255)
     ap.add_argument("-b", action="store_true", help="count k-mers as they are, not canonical ones")
+    ap.add_argument("--hc", action="store_true", help="count homopolymer-compressed k-mers, as kmc -hc does (-e ignores it, as kmc does)")
     ap.add_argument("--batch-bytes", type=int, default=1 << 26)
     ap.add_argument("--device", type=int, default=0)
     ap.add_argument("--gpu-parse", action="store_true", help="parse FASTQ / FASTA on the GPU in chunks of batch-bytes - 1 (default: numpy, whole files)")
@@ -587,13 +604,13 @@ def main(argv=None):
     if a.small_k or a.k <= m:                                           # no bins: no map, and the path picks its own LUT prefix length
         if a.opt_out_size:
             ap.error("histogram estimation is not supported on the small-k path, as in kmc")
-        print(json.dumps(count_reads_small_k(a.inputs[:-1], a.inputs[-1], a.k, a.ci, a.cx, a.cs, not a.b, a.batch_bytes, a.device, parse)))
+        print(json.dumps(count_reads_small_k(a.inputs[:-1], a.inputs[-1], a.k, a.ci, a.cx, a.cs, not a.b, a.batch_bytes, a.device, parse, a.hc)))
         return 0
     lp = a.lut_prefix_len
     if lp is None and not a.opt_out_size:
         lp = next(p for p in (7, 3, 11, 15, 4, 5, 6, 2, 8, 9, 10, 12, 13, 14, 1) if p < a.k and (a.k - p) % 4 == 0)
     res = count_reads(a.inputs[:-1], a.inputs[-1], a.k, m, sig_map, lp, a.ci, a.cx, a.cs, not a.b, a.batch_bytes, a.device,
-                      a.n_bins if sig_map is None else None, parse=parse, small_k=False, opt_out_size=a.opt_out_size)
+                      a.n_bins if sig_map is None else None, parse=parse, small_k=False, opt_out_size=a.opt_out_size, homopolymer_compressed=a.hc)
     print(json.dumps(res))
     return 0
 

@@ -281,7 +281,8 @@ int kmcb200_stage2_bin_order(uint32_t n_bins, const uint64_t* bytes, const uint6
  *   FASTQ  line 1 of every 4 is kept with its '\n'; lines are counted from the chunk's start, so every chunk must start on a record;
  *   FASTA  a header line (first byte '>') becomes one '\n', every other line is kept without its '\n', blank lines vanish.
  * '\r' is an ordinary byte (a separator in the batch).  A final chunk that does not end in '\n' is parsed as if it did, so the output
- * never exceeds bytes + 1.  The format is the caller's choice (the file's first non-empty line starts with '@' or '>'); gzip is not read.
+ * never exceeds bytes + 1.  The format is the caller's choice (the file's first non-empty line starts with '@' or '>'); the parser reads
+ * text only: gzip input is inflated before it (see "gzip input" below).
  * Records end after every 4th line (FASTQ) or where a header line starts after a '\n' (FASTA); the end of a final chunk ends one too.
  *   is_final == 0  the chunk is parsed up to its last record end, returned as `consumed`: the caller carries the rest into the next chunk.
  *                  A chunk without a record end is KMCB200_ERR_INVALID ("a record is longer than the chunk") and nothing else is written.
@@ -420,6 +421,54 @@ int kmcb200_estimator_read(kmcb200_estimator* h, uint32_t* counters);
 /* *n = max_occ + 1 and hist[0, *n) the estimate of the current counters.  capacity < *n: KMCB200_ERR_CAPACITY, *n set, hist not written. */
 int kmcb200_estimator_histogram(kmcb200_estimator* h, uint64_t* hist, uint64_t capacity, uint64_t* n);
 int kmcb200_estimator_reset(kmcb200_estimator* h);
+
+/* ---- gzip input: BGZF members inflated on the GPU (RFC 1951 / 1952; what `bgzip` and `samtools` write) ------------------------------
+ * A BGZF file is a series of independent gzip members: ID1 ID2 = 1f 8b, CM = 8, FLG = FEXTRA alone, an extra field with a 'BC' subfield
+ * (SLEN 2) that holds BSIZE (the member's bytes - 1), the deflate data, then CRC32 and ISIZE (its text bytes, at most 64 KiB).  Every member
+ * is inflated by one warp on its own (kmc_b200/csrc/inflate.cuh), so a call that holds thousands of members keeps the GPU busy.  Any
+ * other gzip stream (plain `gzip`, `pigz`) is one serial stream: kmc_b200.reads inflates those with zlib on its reader thread.
+ * The text is zlib's byte for byte.  A malformed member (invalid codes or code sets, a distance before the member's start, more or less
+ * output than ISIZE, a CRC32 mismatch, a truncated stream, ...) makes the call KMCB200_ERR_INVALID with the member's offset in the
+ * message, and no text of that call is handed on.  No zlib is linked. */
+typedef struct {
+	uint64_t in_off;                      /* the member's first byte in the compressed buffer */
+	uint64_t out_off;                     /* its first text byte: the exclusive sum of the ISIZEs before it */
+	uint32_t in_bytes;                    /* BSIZE + 1 */
+	uint32_t isize;                       /* its text bytes (the trailer's ISIZE) */
+} kmcb200_bgzf_member;
+/* The member walk, host only (no device needed): takes whole BGZF members from raw[0] on while their ISIZE sum fits text_capacity (and, when
+ * members is not NULL, while fewer than members_capacity are taken), and stops before a partial member, a non-BGZF member or one whose ISIZE
+ * is over 64 KiB.  *consumed: the compressed bytes of the members taken, *text_bytes: their text bytes, *n_members: how many; members[0, n)
+ * their table.  KMCB200_ERR_INVALID (message in kmcb200_gunzip_last_error(NULL)) when the first member is not BGZF. */
+int kmcb200_bgzf_scan(const uint8_t* raw, uint64_t bytes, uint64_t text_capacity, kmcb200_bgzf_member* members, uint64_t members_capacity,
+	uint64_t* consumed, uint64_t* text_bytes, uint64_t* n_members);
+typedef struct kmcb200_gunzip kmcb200_gunzip;
+typedef struct {
+	int32_t device;                       /* CUDA ordinal */
+	uint32_t reserved;                    /* 0 */
+	uint64_t max_in_bytes;                /* largest compressed buffer one call accepts (1..KMCB200_SPLIT_MAX_BATCH) */
+	uint64_t max_out_bytes;               /* largest text one call makes (1..KMCB200_SPLIT_MAX_BATCH) */
+} kmcb200_gunzip_params;
+/* KMCB200_ERR_INVALID for a bad parameter, KMCB200_ERR_NO_DEVICE without an sm_90 device (no CPU fallback).  Workspace: max_in_bytes +
+ * max_out_bytes in HBM, and a member table of 24 B per 28 B of max_in_bytes in HBM and in pinned host memory. */
+int kmcb200_gunzip_create(const kmcb200_gunzip_params* params, kmcb200_gunzip** out);
+void kmcb200_gunzip_destroy(kmcb200_gunzip* p);
+/* message of the last failure on this inflater (or of the last failed create or kmcb200_bgzf_scan when p == NULL) */
+const char* kmcb200_gunzip_last_error(const kmcb200_gunzip* p);
+/* Number of kernels this inflater has launched so far (one per call that holds a member). */
+uint64_t kmcb200_gunzip_kernel_launches(const kmcb200_gunzip* p);
+/* Host buffers: the members kmcb200_bgzf_scan takes from raw[0, bytes) with min(text_capacity, max_out_bytes) are copied in, inflated on the
+ * inflater's own stream, and their text copied to text[0, *text_bytes); *consumed: their compressed bytes (0 and 0: not one whole member
+ * fits).  bytes > max_in_bytes or a first member that is not BGZF: KMCB200_ERR_INVALID.  A malformed member: KMCB200_ERR_INVALID, *consumed
+ * = *text_bytes = 0 and text is not written. */
+int kmcb200_gunzip_inflate(kmcb200_gunzip* p, const uint8_t* raw, uint64_t bytes, uint8_t* text, uint64_t text_capacity, uint64_t* consumed,
+	uint64_t* text_bytes);
+/* Device twin: d_members[0, n_members) (a kmcb200_bgzf_scan table, copied to HBM), d_raw[0, raw_bytes) and d_text[0, text_capacity) in
+ * HBM, queued on `stream` (a cudaStream_t; NULL = the legacy default stream) with no host synchronisation.  *d_error (HBM) receives ~0 when
+ * every member is good, else min over the bad members of (member index << 8 | error code); the table is checked against raw_bytes and
+ * text_capacity in the kernel. */
+int kmcb200_dev_gunzip_inflate(kmcb200_gunzip* p, const kmcb200_bgzf_member* d_members, uint64_t n_members, const uint8_t* d_raw, uint64_t raw_bytes,
+	uint8_t* d_text, uint64_t text_capacity, uint64_t* d_error, void* stream);
 
 /* ---- seam #1: sort host records ------------------------------------------------------------------
  * Contract of SortFunction (raduls.h:19-20, kb_sorter.h:775-779): n records of rec_bytes (multiple of 8,

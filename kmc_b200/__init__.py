@@ -55,6 +55,15 @@ class _FastxParams(C.Structure):
     _fields_ = [("device", C.c_int32), ("format", C.c_uint32), ("max_chunk_bytes", C.c_uint64)]
 
 
+class _GunzipParams(C.Structure):
+    _fields_ = [("device", C.c_int32), ("reserved", C.c_uint32), ("max_in_bytes", C.c_uint64), ("max_out_bytes", C.c_uint64)]
+
+
+# kmcb200_bgzf_member: one BGZF member of a call
+BGZF_MEMBER = np.dtype([("in_off", "<u8"), ("out_off", "<u8"), ("in_bytes", "<u4"), ("isize", "<u4")])
+BGZF_MIN_MEMBER = 28                                                    # header, empty deflate block, trailer
+
+
 class BinFragment(C.Structure):
     """kmcb200_bin_fragment: one bin's share of a split batch."""
     _fields_ = [("byte_off", C.c_uint64), ("bytes", C.c_uint64), ("n_rec", C.c_uint64), ("n_super_kmers", C.c_uint64),
@@ -80,6 +89,8 @@ EXPORTS = [
     "kmcb200_estimator_create", "kmcb200_estimator_destroy", "kmcb200_estimator_last_error", "kmcb200_estimator_kernel_launches",
     "kmcb200_estimator_add", "kmcb200_dev_estimator_add", "kmcb200_estimator_add_fastx", "kmcb200_estimator_read",
     "kmcb200_estimator_histogram", "kmcb200_estimator_reset",
+    "kmcb200_bgzf_scan", "kmcb200_gunzip_create", "kmcb200_gunzip_destroy", "kmcb200_gunzip_last_error", "kmcb200_gunzip_kernel_launches",
+    "kmcb200_gunzip_inflate", "kmcb200_dev_gunzip_inflate",
 ]
 
 FASTQ, FASTA = 1, 2                                                     # KMCB200_FASTQ / KMCB200_FASTA
@@ -202,6 +213,16 @@ def load_library(build_if_needed=True):
     L.kmcb200_estimator_read.argtypes = [vp, vp]
     L.kmcb200_estimator_histogram.argtypes = [vp, vp, u64, C.POINTER(u64)]
     L.kmcb200_estimator_reset.argtypes = [vp]
+    L.kmcb200_bgzf_scan.argtypes = [vp, u64, u64, vp, u64, C.POINTER(u64), C.POINTER(u64), C.POINTER(u64)]
+    L.kmcb200_gunzip_create.argtypes = [C.POINTER(_GunzipParams), C.POINTER(vp)]
+    L.kmcb200_gunzip_destroy.argtypes = [vp]
+    L.kmcb200_gunzip_destroy.restype = None
+    L.kmcb200_gunzip_last_error.argtypes = [vp]
+    L.kmcb200_gunzip_last_error.restype = C.c_char_p
+    L.kmcb200_gunzip_kernel_launches.argtypes = [vp]
+    L.kmcb200_gunzip_kernel_launches.restype = u64
+    L.kmcb200_gunzip_inflate.argtypes = [vp, vp, u64, vp, u64, C.POINTER(u64), C.POINTER(u64)]
+    L.kmcb200_dev_gunzip_inflate.argtypes = [vp, vp, u64, vp, u64, vp, u64, vp, vp]
     _lib = L
     return L
 
@@ -743,6 +764,51 @@ class FastxParser(_Handle):
         consumed, sequence bytes, records, error flag (a non-final chunk without a record end)."""
         self._check(self.lib.kmcb200_dev_fastx_parse(self._h, d_raw, nbytes, int(bool(is_final)), FASTX_NO_LIMIT if limit is None else int(limit),
                                                      d_seq, seq_capacity, d_result, stream))
+
+
+class Gunzip(_Handle):
+    """BGZF members inflated on one GPU (kmcb200_gunzip_*): one warp per member, the text zlib's byte for byte, every member's CRC32 and
+    ISIZE checked.  A malformed member raises ERR_INVALID with its offset and leaves text_out unwritten.  Plain (non-BGZF) gzip is serial:
+    kmc_b200.reads inflates it with zlib."""
+    _prefix = "kmcb200_gunzip"
+
+    def __init__(self, device=0, max_in_bytes=1 << 26, max_out_bytes=1 << 26):
+        self.max_in_bytes, self.max_out_bytes = max_in_bytes, max_out_bytes
+        p = _GunzipParams(device, 0, max_in_bytes, max_out_bytes)
+        self._open(C.byref(p))
+
+    def kernel_launches(self):
+        return int(self.lib.kmcb200_gunzip_kernel_launches(self._h))
+
+    def inflate(self, raw, text_out):
+        """kmcb200_gunzip_inflate: the whole BGZF members at the start of raw (at most max_in_bytes, ideally pinned) whose text fits
+        text_out (uint8, ideally pinned) are inflated into it.  Returns (consumed, text_bytes); (0, 0) when not one whole member fits.
+        ERR_INVALID when raw does not start with a BGZF member."""
+        a = _as_u8(raw)
+        consumed, nbytes = C.c_uint64(0), C.c_uint64(0)
+        self._check(self.lib.kmcb200_gunzip_inflate(self._h, a.ctypes.data, a.size, text_out.ctypes.data, text_out.size, C.byref(consumed),
+                                                    C.byref(nbytes)))
+        return int(consumed.value), int(nbytes.value)
+
+    def dev_inflate(self, d_members, n_members, d_raw, raw_bytes, d_text, text_capacity, d_error, stream=None):
+        """kmcb200_dev_gunzip_inflate: device pointers (ints or tensors' data_ptr()); d_members holds a bgzf_scan table; d_error receives ~0,
+        or min over the bad members of (index << 8 | error code)."""
+        self._check(self.lib.kmcb200_dev_gunzip_inflate(self._h, d_members, n_members, d_raw, raw_bytes, d_text, text_capacity, d_error, stream))
+
+
+def bgzf_scan(raw, capacity, max_members=None):
+    """kmcb200_bgzf_scan (host only, no GPU): the whole BGZF members at the start of raw whose text fits `capacity` bytes.  Returns
+    (consumed, text_bytes, members), members a BGZF_MEMBER array (in_off, out_off, in_bytes, isize).  ERR_INVALID when raw does not start
+    with a BGZF member."""
+    lib = load_library()
+    a = _as_u8(raw)
+    cap = a.size // BGZF_MIN_MEMBER + 1 if max_members is None else int(max_members)
+    members = np.zeros(cap, dtype=BGZF_MEMBER)
+    consumed, text, n = C.c_uint64(0), C.c_uint64(0), C.c_uint64(0)
+    rc = lib.kmcb200_bgzf_scan(a.ctypes.data, a.size, int(capacity), members.ctypes.data, cap, C.byref(consumed), C.byref(text), C.byref(n))
+    if rc < 0:
+        raise KmcB200Error(rc, (lib.kmcb200_gunzip_last_error(None) or b"").decode())
+    return int(consumed.value), int(text.value), members[:n.value]
 
 
 def _host_check(lib, rc):

@@ -18,6 +18,7 @@
 #include "hc.cuh"
 #include "small_k.cuh"
 #include "estimate.cuh"
+#include "inflate.cuh"
 
 #include <cmath>
 #include <cstddef>
@@ -1686,3 +1687,4 @@ int kmcb200_leaf_plan(kmcb200_ctx* ctx, uint32_t slot, uint32_t* out)
 #include "fastx.inl"
 #include "small_k.inl"
 #include "estimate.inl"
+#include "gunzip.inl"

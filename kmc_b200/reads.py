@@ -40,6 +40,15 @@ n_super_kmers are counted after compression.  The files are `kmc -hc -sr1`'s for
 longer records into parts and compresses each part on its own (DESIGN.md section 3.13), the GPU compresses every record whole.
 
     python -m kmc_b200.reads --hc -k31 reads.fq out_prefix
+
+gzip input: a file that starts with 1f 8b is gzip (a FASTQ / FASTA text never does), whatever its name, and FASTQ or FASTA is decided on
+its text.  parse="host" inflates the whole file with zlib, every member.  parse="gpu" inflates BGZF members (what `bgzip` writes) on the
+GPU (kmc_b200.Gunzip) on the reader thread, into the chunk behind the carried rest; from the first member that is not BGZF on (plain
+`gzip`, concatenated members) zlib inflates the rest on that thread.  The text is zlib's byte for byte, so the databases, -e files and
+totals are those of the same text uncompressed.  As in the reference, a gzip file counts 3.2 times its bytes in the predicted input size
+(stage 0's sample budget, the estimator's s); the sample itself and the parser's limit count text bytes.
+
+    python -m kmc_b200.reads --gpu-parse -k31 reads.fq.gz out_prefix
 """
 import argparse
 import json
@@ -49,15 +58,67 @@ import struct
 import sys
 import threading
 import time
+import zlib
 
 import numpy as np
 
-from . import DbWriter, FASTA, FASTQ, FastxParser, HistogramEstimator, KmcB200Error, ERR_INVALID, SignatureStats, SmallKCounter, Splitter, \
-    Stage2Context, Stage2Params, signature_map as _signature_map, stage2_bin_order
+from . import DbWriter, FASTA, FASTQ, FastxParser, Gunzip, HistogramEstimator, KmcB200Error, ERR_INVALID, SignatureStats, SmallKCounter, \
+    Splitter, Stage2Context, Stage2Params, bgzf_scan, signature_map as _signature_map, stage2_bin_order
 
 _NL, _GT, _AT = 10, ord(">"), ord("@")
 STATS_SAMPLE_BYTES = 1 << 28                                            # STATS_FASTQ_SIZE (kmc_core/defs.h)
 DEFAULT_N_BINS = 512                                                    # kmc -n
+GZIP_MAGIC = b"\x1f\x8b"
+GZIP_SIZE_FACTOR = 3.2                                                  # binary_reader.h:378-386: a gzip file's predicted text size
+BGZF_MAX_TEXT = 1 << 16                                                 # text of one BGZF member, at most
+_ZLIB_READ = 1 << 18                                                    # compressed bytes per zlib step on the reader thread
+
+
+def is_gzip(path):
+    """The file starts with the gzip magic 1f 8b.  A FASTQ / FASTA text never does (its first byte is '@', '>' or a line break)."""
+    with open(path, "rb") as f:
+        return f.read(2) == GZIP_MAGIC
+
+
+def predicted_size(paths):
+    """The input size the reference plans with (CBinaryFilesReader, binary_reader.h:378-386): a plain file counts its bytes, a gzip file
+    (uint64)(3.2 * its bytes).  The reference tells gzip by the name's ".gz", this library by the file's first bytes."""
+    return sum(int(GZIP_SIZE_FACTOR * os.path.getsize(p)) if is_gzip(p) else os.path.getsize(p) for p in paths)
+
+
+def _gzip_error(e):
+    return KmcB200Error(ERR_INVALID, "gzip input: %s" % e)
+
+
+def _zlib_members(data, more=None):
+    """Text blocks of gzip data with zlib, member after member (inflateReset for each further member, as the reference's reader does).
+    more(): further compressed bytes (b"" at the end of the file).  A member cut short at the end is an error."""
+    d, fresh = zlib.decompressobj(31), True
+    while True:
+        if not data:
+            data = more() if more else b""
+            if not data:
+                if not fresh:
+                    raise _gzip_error("the last member is truncated")
+                return
+        try:
+            t = d.decompress(data)
+        except zlib.error as e:
+            raise _gzip_error(e) from None
+        fresh = False
+        if d.eof:
+            data, d, fresh = d.unused_data, zlib.decompressobj(31), True
+        else:
+            data = b""
+        if t:
+            yield t
+
+
+def read_text(path):
+    """The whole text of a FASTQ / FASTA file, inflated with zlib (every member) when it is gzip."""
+    with open(path, "rb") as f:
+        data = f.read()
+    return b"".join(_zlib_members(data)) if data[:2] == GZIP_MAGIC else data
 
 
 def sequences_to_batch(data):
@@ -149,9 +210,10 @@ class _RawChunks:
     """One file as raw chunks of at most chunk_bytes in pinned host memory, for the GPU parser.  A reader thread fills two pinned buffers
     in turn with the next chunk_bytes / 2 bytes of the file, so reading the next piece overlaps the work on the current chunk.  Iterating
     gives (chunk, is_final); the caller reports how much of each non-final chunk it parsed with .consumed(n), and the rest (an unfinished
-    record) is copied in front of the next piece, so every chunk starts on a record.  close() (or leaving the `with`) ends the thread."""
+    record) is copied in front of the next piece, so every chunk starts on a record.  close() (or leaving the `with`) ends the thread.
+    A gzip file gives its text the same way, chunk_bytes / 2 text bytes per piece (_GzText)."""
 
-    def __init__(self, path, chunk_bytes):
+    def __init__(self, path, chunk_bytes, device=0):
         self.size = os.path.getsize(path)
         self.piece = max(1, chunk_bytes // 2)
         self.head = chunk_bytes - self.piece                           # room for the carried rest of the previous chunk
@@ -162,7 +224,8 @@ class _RawChunks:
         self.wait_s = 0.0                                               # time the consumer waited for the reader
         self._consumed = None
         self._f = open(path, "rb")
-        self._thread = threading.Thread(target=self._read, name="kmc_b200-reader", daemon=True)
+        self._gz = _GzText(self._f, self.piece, device) if is_gzip(path) else None
+        self._thread = threading.Thread(target=self._read if self._gz is None else self._read_gzip, name="kmc_b200-reader", daemon=True)
         self._thread.start()
 
     def _read(self):
@@ -181,6 +244,19 @@ class _RawChunks:
         except BaseException as e:  # noqa: BLE001 - handed to the consumer
             self.full.put(e)
 
+    def _read_gzip(self):
+        try:
+            while True:
+                i = self.free.get()
+                if i is None:
+                    return
+                n, final = self._gz.fill(self.bufs[i][1][self.head:self.head + self.piece])
+                self.full.put((i, n, final))
+                if final:
+                    return
+        except BaseException as e:  # noqa: BLE001 - handed to the consumer
+            self.full.put(e)
+
     def consumed(self, n):
         self._consumed = int(n)
 
@@ -195,6 +271,11 @@ class _RawChunks:
             i, n, final = item
             buf = self.bufs[i][1]
             start = self.head
+            if final and n == 0 and (carry is None or carry[1] == carry[2]):   # a gzip text that ended with the previous piece
+                self.free.put(i)
+                if carry is not None:
+                    self.free.put(carry[0])
+                return
             if carry is not None:
                 j, s, e = carry
                 if e - s > self.head:
@@ -216,6 +297,8 @@ class _RawChunks:
             self.free.put(None)
             self.free.put(None)
             self._thread.join()
+        if self._gz is not None:
+            self._gz.close()
         self._f.close()
 
     def __enter__(self):
@@ -223,6 +306,78 @@ class _RawChunks:
 
     def __exit__(self, *exc):
         self.close()
+
+
+class _GzText:
+    """The text of a gzip file, piece by piece, for _RawChunks' reader thread.  BGZF members are inflated on the GPU (Gunzip, on its own
+    stream, so this overlaps the parse and split of the previous chunk): compressed bytes are read into a pinned buffer, the whole members
+    that fit the piece are inflated straight into it, and a partial member stays for the next read.  From the first member that is not BGZF
+    on (plain `gzip`, concatenated members, or a later part of a mixed file), zlib inflates the rest of the file, member after member."""
+
+    def __init__(self, f, piece, device):
+        self.f, self.piece, self.device = f, piece, device
+        self.zcap = piece + (1 << 17)                                  # a piece of text in members, and the partial member after them
+        self._zt, self.z = _pinned(self.zcap)
+        self.zlen, self.eof = 0, False
+        self.gz = None                                                  # the GPU inflater, created with the first BGZF member
+        self.blocks = None                                              # zlib's text blocks, from the first member that is not BGZF on
+        self.pending, self.pending_off = b"", 0
+
+    def _read_more(self):
+        if not self.eof and self.zlen < self.zcap:
+            n = self.f.readinto(memoryview(self.z)[self.zlen:])
+            self.eof = n < self.zcap - self.zlen
+            self.zlen += n
+
+    def _bgzf_next(self):
+        try:
+            bgzf_scan(self.z[:self.zlen], 0, max_members=1)
+            return True
+        except KmcB200Error:
+            return False
+
+    def fill(self, out):
+        """Text into out[0, n); returns (n, final).  n > 0 unless final."""
+        n = 0
+        while self.blocks is None:
+            self._read_more()
+            if self.zlen == 0:
+                return n, True
+            if not self._bgzf_next():
+                rest = bytes(self.z[:self.zlen])
+                self.zlen = 0
+                self.blocks = _zlib_members(rest, lambda: self.f.read(_ZLIB_READ))
+                break
+            if self.gz is None:
+                if self.piece < BGZF_MAX_TEXT:
+                    raise KmcB200Error(ERR_INVALID, "BGZF input needs pieces of at least 64 KiB of text: batch_bytes of at least %d" %
+                                       (2 * BGZF_MAX_TEXT + 2))
+                self.gz = Gunzip(self.device, self.zcap, self.piece)
+            used, t = self.gz.inflate(self.z[:self.zlen], out[n:])
+            n += t
+            if used:
+                self.z[:self.zlen - used] = self.z[used:self.zlen]
+                self.zlen -= used
+            if self.eof and self.zlen == 0:
+                return n, True
+            if used == 0:
+                if n:
+                    return n, False                                     # the next member does not fit this piece
+                raise _gzip_error("the last BGZF member is truncated")
+        while n < out.size:                                             # zlib
+            if self.pending_off == len(self.pending):
+                self.pending, self.pending_off = next(self.blocks, None), 0
+                if self.pending is None:
+                    return n, True
+            take = min(out.size - n, len(self.pending) - self.pending_off)
+            out[n:n + take] = np.frombuffer(self.pending, dtype=np.uint8, count=take, offset=self.pending_off)
+            n += take
+            self.pending_off += take
+        return n, False
+
+    def close(self):
+        if self.gz is not None:
+            self.gz.close()
 
 
 class _Parsers:
@@ -245,10 +400,11 @@ class _Parsers:
 
 def signature_sample_counts(paths, k, signature_len, batch_bytes=1 << 26, device=0, parse="host", homopolymer_compressed=False):
     """Stage 0's statistics (CKMC::buildSignatureMapping, kmc_core/kmc.h:974-1075): k-mers per signature, counted on the GPU, over the
-    raw bytes of the files in input order up to the end of the first record at or beyond max(2^28, total bytes / 100).
+    text of the files in input order up to the end of the first record at or beyond max(2^28, predicted_size / 100) text bytes (a gzip
+    file counts 3.2 times its bytes in the prediction, its text in the sample).
     parse="gpu": the files are parsed on the GPU in chunks of batch_bytes - 1, the sample's end found by the parser's limit.
     homopolymer_compressed: the k-mers of the compressed reads are counted (`kmc -hc`); the sample's end is still found on the raw bytes."""
-    budget = max(STATS_SAMPLE_BYTES, sum(os.path.getsize(p) for p in paths) // 100)
+    budget = max(STATS_SAMPLE_BYTES, predicted_size(paths) // 100)
     st = SignatureStats(k, signature_len, device, max_batch_bytes=batch_bytes, homopolymer_compressed=homopolymer_compressed)
     if parse == "gpu":
         parsers = _Parsers(device, batch_bytes - 1)
@@ -256,16 +412,16 @@ def signature_sample_counts(paths, k, signature_len, batch_bytes=1 << 26, device
             for path in paths:
                 if budget <= 0:
                     break
-                size, pos = os.path.getsize(path), 0
-                with _RawChunks(path, batch_bytes - 1) as chunks:
+                cut, pos = is_gzip(path) or os.path.getsize(path) > budget, 0     # a gzip text's size is known once it is read
+                with _RawChunks(path, batch_bytes - 1, device) as chunks:
                     parser = None
                     for chunk, final in chunks:
                         parser = parser or parsers(chunk)
-                        limit = budget - pos if size > budget else None
+                        limit = budget - pos if cut else None
                         used = st.add_fastx(parser, chunk, final, limit)
                         chunks.consumed(used)
                         pos += used
-                        if size > budget and pos >= budget:
+                        if cut and pos >= budget:
                             break
                 budget -= pos
         finally:
@@ -276,8 +432,7 @@ def signature_sample_counts(paths, k, signature_len, batch_bytes=1 << 26, device
     for path in paths:
         if budget <= 0:
             break
-        with open(path, "rb") as f:
-            data = f.read()
+        data = read_text(path)
         if not data:
             continue
         if len(data) > budget:
@@ -296,8 +451,9 @@ ESTIMATE_LARGE_INPUT = 50_000_000_000                                   # kmc.h:
 
 
 def estimate_s(paths):
-    """The reference's sampling exponent for these inputs: 7, or 11 when the files hold at least 5 * 10^10 bytes."""
-    return 11 if sum(os.path.getsize(p) for p in paths) >= ESTIMATE_LARGE_INPUT else 7
+    """The reference's sampling exponent for these inputs: 7, or 11 when their predicted size (predicted_size: gzip files count 3.2 times
+    their bytes) is at least 5 * 10^10 bytes."""
+    return 11 if predicted_size(paths) >= ESTIMATE_LARGE_INPUT else 7
 
 
 def n_records(data):
@@ -348,14 +504,13 @@ def estimate_histogram(paths, k, s=None, batch_bytes=1 << 26, device=0, parse="h
     try:
         for path in paths:
             if parsers is not None:
-                with _RawChunks(path, batch_bytes - 1) as chunks:
+                with _RawChunks(path, batch_bytes - 1, device) as chunks:
                     parser = None
                     for chunk, final in chunks:
                         parser = parser or parsers(chunk)
                         chunks.consumed(est.add_fastx(parser, chunk, final))
                 continue
-            with open(path, "rb") as f:
-                data = f.read()
+            data = read_text(path)
             if not data:
                 continue
             for batch in batches(sequences_to_batch(data), batch_bytes):
@@ -392,7 +547,7 @@ def count_reads_small_k(paths, out_prefix, k, cutoff_min=2, cutoff_max=1_000_000
     try:
         for path in paths:
             if parsers is not None:
-                with _RawChunks(path, batch_bytes - 1) as chunks:
+                with _RawChunks(path, batch_bytes - 1, device) as chunks:
                     parser = None
                     for chunk, final in chunks:
                         parser = parser or parsers(chunk)
@@ -401,8 +556,7 @@ def count_reads_small_k(paths, out_prefix, k, cutoff_min=2, cutoff_max=1_000_000
                 read_s += chunks.wait_s
                 continue
             t = time.perf_counter()
-            with open(path, "rb") as f:
-                data = f.read()
+            data = read_text(path)
             read_s += time.perf_counter() - t
             seq = sequences_to_batch(data)
             del data
@@ -486,7 +640,7 @@ def count_reads(paths, out_prefix, k, signature_len, signature_map, lut_prefix_l
     try:
         for path in paths:
             if parsers is not None:
-                with _RawChunks(path, batch_bytes - 1) as chunks:
+                with _RawChunks(path, batch_bytes - 1, device) as chunks:
                     parser = None
                     for chunk, final in chunks:
                         parser = parser or parsers(chunk)
@@ -502,8 +656,7 @@ def count_reads(paths, out_prefix, k, signature_len, signature_map, lut_prefix_l
                 read_s += chunks.wait_s
                 continue
             t = time.perf_counter()
-            with open(path, "rb") as f:
-                data = f.read()
+            data = read_text(path)
             read_s += time.perf_counter() - t
             n_reads += n_records(data)
             seq = sequences_to_batch(data)

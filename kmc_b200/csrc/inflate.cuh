@@ -16,10 +16,11 @@
 //
 // Validation (a bad member sets the call's error word to min(member << 8 | code), and the call returns KMCB200_ERR_INVALID):
 //   every input byte read is inside the member's deflate data (past its end the bit reader shifts in zeros, and a stream that consumed
-//   them is truncated), every output byte and every back-reference inside [0, ISIZE) of the member's slice; invalid block types, stored
-//   lengths whose complement does not match, over-subscribed code sets and the incomplete ones zlib's inflate_table rejects, codes with no
-//   symbol, length / distance symbols 286-287 / 30-31, a repeat with no previous length, a dynamic header without end-of-block, a stream
-//   that ends before its final block or leaves bytes before the trailer, and CRC32 / ISIZE mismatches.
+//   them is truncated, whatever error those zeros would give), every output byte and every back-reference inside [0, ISIZE) of the
+//   member's slice; invalid block types, stored lengths whose complement does not match, over-subscribed code sets and the incomplete
+//   ones zlib's inflate_table rejects, codes with no symbol, length / distance symbols 286-287 / 30-31, a repeat with no previous length,
+//   a dynamic header without end-of-block, a stream that ends before its final block or leaves bytes before the trailer, and CRC32 /
+//   ISIZE mismatches.  Each error is the one zlib reports for the same deflate data.
 #pragma once
 #include <cstdint>
 
@@ -171,7 +172,8 @@ struct GzBits {
 	__device__ uint64_t consumed() const { return ip * 8 - nb; }
 };
 
-// a symbol of table t (lookup of `bits` bits, then code by code up to 15 bits); needs >= 15 bits in the reader.  ~0u: no such code.
+// a symbol of table t (lookup of `bits` bits, then code by code up to 15 bits); needs >= 15 bits in the reader.  ~0u: no such code, which
+// only an empty set or a single 1-bit code has; the one bit is consumed, as zlib's table for such a set consumes it.
 __device__ __forceinline__ uint32_t gz_decode(GzBits& r, const GzTable& t, const uint16_t* tab, uint32_t bits)
 {
 	const uint16_t e = tab[r.peek(bits)];
@@ -185,6 +187,7 @@ __device__ __forceinline__ uint32_t gz_decode(GzBits& r, const GzTable& t, const
 		first = (first + c) << 1;
 		code <<= 1;
 	}
+	r.drop(1);
 	return ~0u;
 }
 
@@ -215,8 +218,8 @@ __device__ uint32_t gz_read_lengths(GzWarp& s, GzBits& r, uint32_t n)
 	uint32_t i = 0;
 	while (i < n) {
 		r.refill();
-		const uint32_t sym = gz_decode(r, s.lt, s.ltab, 7);
-		if (sym == ~0u) return kGzErrCode;
+		uint32_t sym = gz_decode(r, s.lt, s.ltab, 7);
+		if (sym == ~0u) sym = 0;                                        // an empty code-length code: zlib reads every length as 0
 		if (sym < 16) { s.lens[i++] = (uint8_t)sym; continue; }
 		uint32_t rep, val = 0;
 		if (sym == 16) {
@@ -311,6 +314,10 @@ __device__ uint32_t gz_member(GzWarp& s, const uint32_t* s_crc, const uint8_t* _
 
 	GzBits r{raw, m.in_off + 12 + xlen, m.in_off + m.in_bytes - kGzTrailer, 0, 0};
 	uint32_t op = 0;
+	// lane 0's verdict on an error: one found after the reader consumed bits past the member's data came from the zeros shifted in there,
+	// so the data ended early (zlib reports such a stream unfinished, whatever those zeros decode to).  The reader stops where an error is
+	// found, so consumed() is what the decision needed.
+	const auto failed = [&](uint32_t e) { return lane == 0 && r.consumed() > r.end * 8 ? (uint32_t)kGzErrTruncated : e; };
 	if (lane == 0) { s.err = 0; s.fixed = 0; }
 	__syncwarp();
 	for (;;) {
@@ -327,19 +334,21 @@ __device__ uint32_t gz_member(GzWarp& s, const uint32_t* s_crc, const uint8_t* _
 				if (len != (~nlen & 0xffff)) err = kGzErrStored;
 				else if (at + len > r.end) err = kGzErrTruncated;
 				else if (op + len > isize) err = kGzErrOutput;
-				s.copy_src = at;
-				s.copy_dst = op;
-				s.copy_len = len;
-				r.ip = at + len;
-				r.nb = 0;
-				r.bb = 0;
-				op += len;
+				if (!err) {
+					s.copy_src = at;
+					s.copy_dst = op;
+					s.copy_len = len;
+					r.ip = at + len;
+					r.nb = 0;
+					r.bb = 0;
+					op += len;
+				}
 			} else if (!err && s.btype == 2) {
 				r.refill();
 				const uint32_t hlit = r.take(5) + 257, hdist = r.take(5) + 1, hclen = r.take(4) + 4;
 				if (hlit > 286 || hdist > 30) err = kGzErrCodeSet;
 				for (uint32_t i = 0; i < 19; ++i) s.cl_lens[i] = 0;
-				for (uint32_t i = 0; i < hclen; ++i) {
+				for (uint32_t i = 0; !err && i < hclen; ++i) {
 					r.refill();
 					s.cl_lens[c_gz_clorder[i]] = (uint8_t)r.take(3);
 				}
@@ -349,7 +358,7 @@ __device__ uint32_t gz_member(GzWarp& s, const uint32_t* s_crc, const uint8_t* _
 			s.err = err;
 		}
 		__syncwarp();
-		if (s.err) return s.err;
+		if (s.err) return failed(s.err);
 		const uint32_t btype = s.btype;
 		if (btype == 0) {
 			const uint64_t src = s.copy_src;
@@ -379,7 +388,7 @@ __device__ uint32_t gz_member(GzWarp& s, const uint32_t* s_crc, const uint8_t* _
 				}
 				if (!err) err = gz_build(s, s.lens, hlit, s.lt, s.ltab, kGzLBits, false, lane);
 				if (!err) err = gz_build(s, s.lens + hlit, hdist, s.dt, s.dtab, kGzDBits, false, lane);
-				if (err) return err;
+				if (err) return failed(err);
 			}
 			for (;;) {                                                  // the block's tokens, round by round
 				if (lane == 0) s.err = gz_decode_round(s, r, op, isize);
@@ -387,7 +396,7 @@ __device__ uint32_t gz_member(GzWarp& s, const uint32_t* s_crc, const uint8_t* _
 				gz_write_round(s, out, lane);
 				const uint32_t err = s.err, eob = s.eob;
 				__syncwarp();                                           // read before lane 0 writes the next round
-				if (err) return err;
+				if (err) return failed(err);
 				if (eob) break;
 			}
 		}

@@ -18,6 +18,14 @@
  * thread at a time (KMC runs one sorter thread per context).  There is NO CPU fallback: without a usable
  * sm_90 device kmcb200_create fails with KMCB200_ERR_NO_DEVICE.
  *
+ * Ordering (every handle, and every slot of a stage-2 context): a device-form call (kmcb200_dev_*) is queued on the caller's
+ * stream and returns at once; the handle (slot) records where that work ends, and every later call on the same handle (slot),
+ * device or host form, on any stream, starts on the GPU only after it.  Host-form calls are done when they return (submit_bin:
+ * once wait_bin has returned).  So the handle's own workspace is never shared by two calls at once, and the caller orders only
+ * its own buffers: the inputs it fills before a device-form call and the outputs it reads after one.  Different handles and
+ * different contexts are independent: each may be driven by its own host thread, all at once; one handle or context is still
+ * used by one host thread at a time (its slots included).  The inflater's device twin uses no workspace of its handle.
+ *
  * Environment knobs read by kmcb200_create (development / tests; the defaults are the measured best):
  *   KMCB200_SORT=lsd               plain 8-bit LSD passes instead of the hybrid MSD sort
  *   KMCB200_LEAF_KERNEL=cta|hash   one-word records always by one table per CTA (leaf_hash_cta_kernel) / one table per warp (leaf_hash_kernel);

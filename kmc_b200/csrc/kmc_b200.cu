@@ -109,6 +109,7 @@ struct Slot {
 	// events
 	cudaEvent_t ev_begin = nullptr, ev_expand = nullptr, ev_sort = nullptr, ev_count = nullptr, ev_result = nullptr;
 	cudaEvent_t ev_h2d = nullptr, ev_done = nullptr, ev_walk = nullptr;           // copy stream <-> compute stream hand-over
+	cudaEvent_t last = nullptr;                             // end of the slot's latest call, on whichever stream it ran (kmc_b200.h: ordering)
 	cudaEvent_t ev_pass[kMaxPasses + 8] = {};
 	int n_passes_run = 0;                                   // number of timed sort intervals (ev_pass[i] .. ev_pass[i+1])
 	uint32_t leaf_b2 = 0, leaf_kernel = 0;                  // counted leaves of the last bin: level-2 bits, kernel (kmcb200_leaf_plan; 0: not counted)
@@ -1159,7 +1160,7 @@ int kmcb200_create(const kmcb200_params* prm, kmcb200_ctx** out_ctx)
 	if (cudaStreamCreateWithFlags(&ctx->compute, cudaStreamNonBlocking) != cudaSuccess) return bail(fail(ctx, KMCB200_ERR_CUDA, "cudaStreamCreate failed"));
 	for (auto& s : ctx->slots) {
 		bool ok = cudaStreamCreateWithFlags(&s.stream, cudaStreamNonBlocking) == cudaSuccess;
-		for (cudaEvent_t* e : {&s.ev_h2d, &s.ev_done, &s.ev_walk}) ok = ok && cudaEventCreateWithFlags(e, cudaEventDisableTiming) == cudaSuccess;
+		for (cudaEvent_t* e : {&s.ev_h2d, &s.ev_done, &s.ev_walk, &s.last}) ok = ok && cudaEventCreateWithFlags(e, cudaEventDisableTiming) == cudaSuccess;
 		ok = ok && s.zero.alloc(1) == cudaSuccess;
 		ok = ok && cudaMemset(s.zero, 0, sizeof(ZeroBlock)) == cudaSuccess;
 		ok = ok && s.d_lut.alloc(ctx->lut_entries) == cudaSuccess;
@@ -1189,7 +1190,7 @@ void kmcb200_destroy(kmcb200_ctx* ctx)
 	cudaDeviceSynchronize();
 	for (auto& s : ctx->slots) {
 		for (auto e : s.ev_pack) if (e) cudaEventDestroy(e);
-		for (cudaEvent_t e : {s.ev_begin, s.ev_expand, s.ev_sort, s.ev_count, s.ev_result, s.ev_h2d, s.ev_done, s.ev_walk}) if (e) cudaEventDestroy(e);
+		for (cudaEvent_t e : {s.ev_begin, s.ev_expand, s.ev_sort, s.ev_count, s.ev_result, s.ev_h2d, s.ev_done, s.ev_walk, s.last}) if (e) cudaEventDestroy(e);
 		for (auto e : s.ev_pass) if (e) cudaEventDestroy(e);
 		if (s.stream) cudaStreamDestroy(s.stream);
 	}
@@ -1255,6 +1256,8 @@ static int submit_bin_impl(kmcb200_ctx* ctx, uint32_t slot, const uint8_t* super
 	s.have_extras = false;
 	if ((size && !superkmers) || !lut || (!out_suffix && out_capacity)) return fail(ctx, KMCB200_ERR_INVALID, "null buffer");
 	if (int rc = set_device(ctx)) return rc;
+	CU(ctx, cudaStreamWaitEvent(ctx->compute, s.last, 0));
+	CU(ctx, cudaStreamWaitEvent(s.stream, s.last, 0));
 	if (n_rec > ctx->max_block_records || size >= 4 * ctx->max_chunk_bytes) {        // oversized: counted key block by key block, synchronously
 		CU(ctx, cudaStreamSynchronize(ctx->compute));
 		if (int rc = run_oversized_bin(ctx, s, superkmers, size, n_rec, pack_bytes, n_packs, out_suffix, out_capacity, lut, &s.sync_out_bytes, s.sync_stats)) return rc;
@@ -1289,6 +1292,7 @@ static int submit_bin_impl(kmcb200_ctx* ctx, uint32_t slot, const uint8_t* super
 		st)) return rc;
 	CU(ctx, cudaGetLastError());
 	CU(ctx, cudaEventRecord(s.ev_result, ctx->compute));
+	CU(ctx, cudaEventRecord(s.last, ctx->compute));
 	s.busy = true;
 	s.host_out = out_suffix; s.host_out_cap = out_capacity; s.host_lut = lut; s.pending_n_rec = n_rec;
 	return 0;
@@ -1406,6 +1410,7 @@ int kmcb200_process_bin_multi(kmcb200_ctx* const* ctxs, uint32_t n_ctx, int32_t 
 		Slot& s = ctx->slots[0];
 		Part& P = parts[g];
 		if (int rc = set_device(ctx)) return rc;
+		CU(ctx, cudaStreamWaitEvent(ctx->compute, s.last, 0));
 		if (P.npacks == 0) { P.hist.assign(4096, 0); return 0; }
 		uint64_t dev_bytes = 0;
 		if (int rc = plan_chunks(ctx, P.bytes, pack_bytes + P.pack0, P.npacks, P.chunks, &dev_bytes)) return rc;
@@ -1563,6 +1568,7 @@ int kmcb200_sort_records(kmcb200_ctx* ctx, void* recs, void* tmp, uint64_t n, ui
 	const int where = (key_bytes & 1) ? 1 : 0;      // kb_sorter.h:776-779
 	if (n == 0) return where;
 	cudaStream_t st = ctx->compute;
+	CU(ctx, cudaStreamWaitEvent(st, s.last, 0));
 	if (int rc = grow(ctx, s.recs_a, n * rec_bytes, kSlotSlack)) return rc;
 	if (int rc = grow(ctx, s.recs_b, n * rec_bytes, kSlotSlack)) return rc;
 	CU(ctx, cudaMemcpyAsync(s.recs_a, recs, n * rec_bytes, cudaMemcpyHostToDevice, st));
@@ -1581,7 +1587,11 @@ int kmcb200_dev_process_bin(kmcb200_ctx* ctx, uint32_t slot, const uint8_t* d_su
 	if (int rc = set_device(ctx)) return rc;
 	Slot& s = ctx->slots[slot];
 	s.have_extras = false;          // (a length-byte array of an earlier kmcb200_submit_bin_indexed on this slot does not describe this bin)
-	return run_bin(ctx, s, d_superkmers, size, n_rec, pack_bytes, n_packs, d_out, out_capacity, d_lut, d_result, stream ? (cudaStream_t)stream : ctx->compute);
+	cudaStream_t st = stream ? (cudaStream_t)stream : ctx->compute;
+	CU(ctx, cudaStreamWaitEvent(st, s.last, 0));
+	if (int rc = run_bin(ctx, s, d_superkmers, size, n_rec, pack_bytes, n_packs, d_out, out_capacity, d_lut, d_result, st)) return rc;
+	CU(ctx, cudaEventRecord(s.last, st));
+	return 0;
 }
 
 int kmcb200_dev_expand(kmcb200_ctx* ctx, uint32_t slot, const uint8_t* d_superkmers, uint64_t size, uint64_t n_rec,
@@ -1593,6 +1603,7 @@ int kmcb200_dev_expand(kmcb200_ctx* ctx, uint32_t slot, const uint8_t* d_superkm
 	cudaStream_t st = stream ? (cudaStream_t)stream : ctx->compute;
 	if (n_rec == 0) return 0;
 	s.have_extras = false;
+	CU(ctx, cudaStreamWaitEvent(st, s.last, 0));
 	CU(ctx, cudaEventRecord(s.ev_begin, st));
 	if (int rc = stage_expand(ctx, s, d_superkmers, size, n_rec, pack_bytes, n_packs, d_recs, st)) return rc;
 	if (d_result) {
@@ -1601,6 +1612,7 @@ int kmcb200_dev_expand(kmcb200_ctx* ctx, uint32_t slot, const uint8_t* d_superkm
 		ctx->launches++;
 	}
 	CU(ctx, cudaEventRecord(s.ev_expand, st));
+	CU(ctx, cudaEventRecord(s.last, st));
 	s.ran_expand = true; s.ran_sort = s.ran_count = false;
 	return 0;
 }
@@ -1614,10 +1626,12 @@ int kmcb200_dev_sort(kmcb200_ctx* ctx, uint32_t slot, void* d_recs, void* d_tmp,
 	cudaStream_t st = stream ? (cudaStream_t)stream : ctx->compute;
 	const int where = (key_bytes & 1) ? 1 : 0;
 	if (n == 0) return where;
+	CU(ctx, cudaStreamWaitEvent(st, s.last, 0));
 	if (!hist_ready) CU(ctx, cudaEventRecord(s.ev_expand, st));
 	bool in_b = false;
 	if (int rc = DISPATCH_WORDS(ctx, launch_sort, ctx, s, d_recs, d_tmp, n, key_bytes, hist_ready ? 2u * ctx->prm.kmer_len : 8u * key_bytes, hist_ready ? s.hist_mode : (int)kHistNone, s.last_n_packs, st, &in_b)) return rc;
 	CU(ctx, cudaEventRecord(s.ev_sort, st));
+	CU(ctx, cudaEventRecord(s.last, st));
 	s.ran_sort = true; s.ran_count = false;
 	if (!hist_ready) s.ran_expand = false;
 	return in_b ? 1 : 0;
@@ -1630,11 +1644,13 @@ int kmcb200_dev_count(kmcb200_ctx* ctx, uint32_t slot, const void* d_sorted, uin
 	if (int rc = set_device(ctx)) return rc;
 	Slot& s = ctx->slots[slot];
 	cudaStream_t st = stream ? (cudaStream_t)stream : ctx->compute;
+	CU(ctx, cudaStreamWaitEvent(st, s.last, 0));
 	CU(ctx, cudaEventRecord(s.ev_sort, st));
 	if (int rc = stage_count(ctx, s, d_sorted, n, d_out, out_capacity, d_lut, d_result, st)) return rc;
 	finish_result_kernel<<<1, 32, 0, st>>>(d_result, n, nullptr, nullptr, nullptr);
 	ctx->launches++;
 	CU(ctx, cudaEventRecord(s.ev_count, st));
+	CU(ctx, cudaEventRecord(s.last, st));
 	s.ran_count = true; s.ran_expand = false; s.ran_sort = false;
 	return 0;
 }

@@ -314,6 +314,62 @@ def expected_from_counts(cnt, p: Params):
     return bytes(out), lut, (n_unique, n_min, n_max, n_total)
 
 
+def emit_rows(suffix, prefixes, counts, p: Params):
+    """(payload bytes, lut, stats) from rows in key order: suffix [m, (k-p)/4] uint8 (most significant byte first), the LUT prefix and the
+    count of every distinct k-mer.  Applies the cutoffs and counter_max as expected_from_counts does, without a Python loop."""
+    counts = np.asarray(counts, dtype=np.uint64)
+    is_min = counts < p.cutoff_min
+    is_max = counts > p.cutoff_max
+    keep = ~(is_min | is_max)
+    kb, cb = suffix.shape[1], p.counter_bytes
+    rows = np.empty((int(keep.sum()), kb + cb), dtype=np.uint8)
+    rows[:, :kb] = suffix[keep]
+    if cb:
+        c = np.minimum(counts[keep], np.uint64(p.counter_max)).astype("<u8")
+        rows[:, kb:] = c.view(np.uint8).reshape(-1, 8)[:, :cb]
+    lut = np.bincount(np.asarray(prefixes)[keep].astype(np.int64), minlength=p.lut_entries).astype(np.uint64)
+    return rows.tobytes(), lut, (int(counts.size), int(is_min.sum()), int(is_max.sum()), int(counts.sum()))
+
+
+def expected_from_arrays(keys, counts, p: Params):
+    """expected_from_counts for k <= 32 on arrays: keys uint64 ascending and distinct, counts uint64 of the same length."""
+    assert p.k <= 32
+    keys = np.asarray(keys, dtype=np.uint64)
+    kb = (p.k - p.lut_prefix_len) // 4
+    suffix = np.empty((keys.size, kb), dtype=np.uint8)
+    for j in range(kb):
+        suffix[:, j] = (keys >> np.uint64(8 * (kb - 1 - j))) & np.uint64(0xFF)
+    return emit_rows(suffix, keys >> np.uint64(8 * kb), counts, p)
+
+
+def raw_params(k, both_strands, lut_prefix_len):
+    """Parameters under which the oracle drops no k-mer and clamps no counter: its output is every distinct k-mer with its exact count."""
+    return Params(k, both_strands, cutoff_min=1, cutoff_max=2 ** 32 - 1, counter_max=2 ** 32 - 1, lut_prefix_len=lut_prefix_len)
+
+
+def raw_rows(oracle, bin_, both_strands, lut_prefix_len):
+    """The oracle's raw counts of a bin as arrays in key order: (suffix [m, (k-p)/4] uint8, prefix uint64 [m], count uint64 [m])."""
+    p = raw_params(bin_.k, both_strands, lut_prefix_len)
+    r = oracle.process_bin(bin_, p)
+    kb = (p.k - p.lut_prefix_len) // 4
+    rows = np.frombuffer(r.payload, dtype=np.uint8).reshape(-1, kb + 4)
+    counts = rows[:, kb:].copy().view("<u4").reshape(-1).astype(np.uint64)
+    prefixes = np.repeat(np.arange(p.lut_entries, dtype=np.uint64), r.lut.astype(np.int64))
+    assert prefixes.size == counts.size == r.stats[0]
+    return rows[:, :kb], prefixes, counts
+
+
+def raw_counts(oracle, bin_, both_strands, lut_prefix_len):
+    """raw_rows as (keys uint64 ascending, counts uint64) for k <= 32: key = (prefix << 8 (k-p)/4) | big-endian suffix."""
+    assert bin_.k <= 32
+    suffix, prefixes, counts = raw_rows(oracle, bin_, both_strands, lut_prefix_len)
+    keys = prefixes.copy()
+    for j in range(suffix.shape[1]):
+        keys <<= np.uint64(8)
+        keys |= suffix[:, j]
+    return keys, counts
+
+
 def decode_payload(payload, lut, p: Params):
     """Inverse of the emit format: list of (kmer string, count) in file order (kmc_api/kmc_file.cpp reader logic)."""
     kb = (p.k - p.lut_prefix_len) // 4

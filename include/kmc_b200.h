@@ -298,14 +298,35 @@ int kmcb200_stage2_bin_order(uint32_t n_bins, const uint64_t* bytes, const uint6
  *                  chunk has one; a non-final chunk without one is parsed to its last record end, so consumed < limit says "go on").
  *                  KMCB200_FASTX_NO_LIMIT (or any limit >= bytes): no cut.
  * Work per call: 9 kernel launches whatever the size, no host synchronisation inside (consumed, the cut and the error are decided on the
- * device).  Workspace: the chunk and the output of the host-buffer form (2 B per byte of max_chunk_bytes) plus 120 B per 16 KiB tile. */
+ * device).  Workspace: the chunk and the output of the host-buffer form (2 B per byte of max_chunk_bytes) plus 120 B per 16 KiB tile.
+ *
+ * BAM (`kmc -fbam`, CSplitter::GetSeq, kmc_core/splitter.cpp:326-418): the chunk is *decompressed* BAM record bytes that start on a record
+ * (the caller inflates the BGZF members and skips the header: magic, l_text, text, n_ref and the references).  A record's bytes may be
+ * split across calls only through `consumed` and the caller's carry, as for FASTQ.
+ *   KMCB200_BAM                  every record whose FLAG has neither 0x100 (secondary) nor 0x800 (supplementary) becomes its l_seq SEQ
+ *                                bases as stored, A C G T for the codes 1 2 4 8 and N for every other code ('=' and IUPAC codes
+ *                                included), then one '\n'; other records add nothing.  What `kmc -fbam` counts.
+ *   KMCB200_BAM_ORIGINAL_STRAND  the same, with the records of FLAG 0x10 reverse complemented back to their original strand: what
+ *                                `kmc -b -fbam` counts.
+ * A record is at least 36 + ceil(l_seq / 2) + l_seq bytes, so the output never exceeds `bytes`; d_result[2] counts the kept records.
+ * Record ends are the ends of BAM records; is_final, limit and consumed mean what they mean above, except that a final chunk that ends
+ * inside a record has no implicit terminator.  A nonzero d_result[3] (then [0..2] are 0 and d_seq is not written; the host forms return
+ * KMCB200_ERR_INVALID) is 1: a non-final chunk without a whole record; 2: a final chunk that ends inside a record (truncated); 3: a
+ * malformed record, block_size < 32, l_seq < 0, or 32 + l_read_name + 4 * n_cigar_op + ceil(l_seq / 2) + l_seq > block_size.
+ * Work per call: 7 kernel launches whatever the size, no host synchronisation inside.  The record walk is parallel where each 16 KiB
+ * tile's guessed first record holds; records that defeat the guesses (no NUL-terminated name, or crafted contents) are walked serially,
+ * about 0.5 us per record on an H100 (DESIGN.md section 3.15).  Workspace: as above, plus 16 B per 36 B of
+ * max_chunk_bytes (0.45 B per byte) for the kept records' starts and output offsets, allocated for a BAM parser only. */
 #define KMCB200_FASTQ 1
 #define KMCB200_FASTA 2
+/* 3 is not a format: it stays refused, as it was before the BAM formats */
+#define KMCB200_BAM 4
+#define KMCB200_BAM_ORIGINAL_STRAND 5
 #define KMCB200_FASTX_NO_LIMIT (~0ull)
 typedef struct kmcb200_fastx kmcb200_fastx;
 typedef struct {
 	int32_t device;                       /* CUDA ordinal */
-	uint32_t format;                      /* KMCB200_FASTQ or KMCB200_FASTA */
+	uint32_t format;                      /* KMCB200_FASTQ, KMCB200_FASTA, KMCB200_BAM or KMCB200_BAM_ORIGINAL_STRAND */
 	uint64_t max_chunk_bytes;             /* largest chunk one call accepts (1..KMCB200_SPLIT_MAX_BATCH): sizes the workspace */
 } kmcb200_fastx_params;
 /* KMCB200_ERR_INVALID for a bad parameter, KMCB200_ERR_NO_DEVICE without an sm_90 device (no CPU fallback). */
@@ -315,13 +336,15 @@ void kmcb200_fastx_destroy(kmcb200_fastx* p);
 const char* kmcb200_fastx_last_error(const kmcb200_fastx* p);
 /* Number of kernels this parser has launched so far (the _fastx entry points below count theirs here too). */
 uint64_t kmcb200_fastx_kernel_launches(const kmcb200_fastx* p);
+/* Records parsed by the latest host-buffer call on this parser (kmcb200_fastx_parse or a _fastx entry point below): d_result[2]. */
+uint64_t kmcb200_fastx_last_records(const kmcb200_fastx* p);
 /* Host buffers: copies the chunk in, returns when seq[0, *seq_bytes) holds the batch and *consumed the bytes parsed.  When the batch is
  * longer than seq_capacity: KMCB200_ERR_CAPACITY, *consumed / *seq_bytes are set and seq is not written. */
 int kmcb200_fastx_parse(kmcb200_fastx* p, const uint8_t* raw, uint64_t bytes, int is_final, uint64_t limit,
 	uint8_t* seq, uint64_t seq_capacity, uint64_t* consumed, uint64_t* seq_bytes);
 /* Device twin: d_raw / d_seq / d_result in HBM, queued on `stream` (a cudaStream_t; NULL = the legacy default stream).  seq_capacity
  * must be at least bytes + 1 (KMCB200_ERR_INVALID otherwise).  d_result receives 4 x uint64: [0] consumed, [1] sequence bytes, [2] records
- * parsed, [3] 1 when a non-final chunk has no record end (then [0..2] are 0 and d_seq is not written). */
+ * parsed, [3] 1 when a non-final chunk has no record end, for BAM also 2 or 3 as above (then [0..2] are 0 and d_seq is not written). */
 int kmcb200_dev_fastx_parse(kmcb200_fastx* p, const uint8_t* d_raw, uint64_t bytes, int is_final, uint64_t limit,
 	uint8_t* d_seq, uint64_t seq_capacity, uint64_t* d_result, void* stream);
 /* kmcb200_split of a raw chunk: copies it in and parses it straight into the splitter's batch buffer, then continues exactly like

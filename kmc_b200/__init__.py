@@ -82,7 +82,7 @@ EXPORTS = [
     "kmcb200_sigstats_create", "kmcb200_sigstats_destroy", "kmcb200_sigstats_last_error", "kmcb200_sigstats_add", "kmcb200_dev_sigstats_add",
     "kmcb200_sigstats_read", "kmcb200_sigstats_reset", "kmcb200_sigstats_kernel_launches", "kmcb200_signature_map", "kmcb200_stage2_bin_order",
     "kmcb200_fastx_create", "kmcb200_fastx_destroy", "kmcb200_fastx_last_error", "kmcb200_fastx_kernel_launches", "kmcb200_fastx_parse",
-    "kmcb200_dev_fastx_parse", "kmcb200_split_fastx", "kmcb200_sigstats_add_fastx",
+    "kmcb200_fastx_last_records", "kmcb200_dev_fastx_parse", "kmcb200_split_fastx", "kmcb200_sigstats_add_fastx",
     "kmcb200_smallk_create", "kmcb200_smallk_destroy", "kmcb200_smallk_last_error", "kmcb200_smallk_kernel_launches", "kmcb200_smallk_add",
     "kmcb200_dev_smallk_add", "kmcb200_smallk_add_fastx", "kmcb200_smallk_read", "kmcb200_smallk_reset", "kmcb200_smallk_finish",
     "kmcb200_smallk_emit", "kmcb200_smallk_write_db",
@@ -93,7 +93,7 @@ EXPORTS = [
     "kmcb200_gunzip_inflate", "kmcb200_dev_gunzip_inflate",
 ]
 
-FASTQ, FASTA = 1, 2                                                     # KMCB200_FASTQ / KMCB200_FASTA
+FASTQ, FASTA, BAM, BAM_ORIGINAL_STRAND = 1, 2, 4, 5                    # KMCB200_FASTQ / _FASTA / _BAM / _BAM_ORIGINAL_STRAND
 FASTX_NO_LIMIT = (1 << 64) - 1
 
 _lib = None
@@ -181,6 +181,8 @@ def load_library(build_if_needed=True):
     L.kmcb200_fastx_last_error.restype = C.c_char_p
     L.kmcb200_fastx_kernel_launches.argtypes = [vp]
     L.kmcb200_fastx_kernel_launches.restype = u64
+    L.kmcb200_fastx_last_records.argtypes = [vp]
+    L.kmcb200_fastx_last_records.restype = u64
     L.kmcb200_fastx_parse.argtypes = [vp, vp, u64, C.c_int, u64, vp, u64, C.POINTER(u64), C.POINTER(u64)]
     L.kmcb200_dev_fastx_parse.argtypes = [vp, vp, u64, C.c_int, u64, vp, u64, vp, vp]
     L.kmcb200_split_fastx.argtypes = [vp, vp, vp, u64, C.c_int, vp, u64, C.POINTER(u64), vp, u64, C.POINTER(u64), vp, C.POINTER(u64), C.POINTER(u64)]
@@ -732,7 +734,9 @@ def _as_u8(raw):
 class FastxParser(_Handle):
     """Reads text -> batch on one GPU (kmcb200_fastx_*): raw FASTQ or FASTA chunks become the batches Splitter and SignatureStats take,
     byte for byte what kmc_b200.reads.sequences_to_batch makes of the whole file.  `fmt` is FASTQ / FASTA (or "fastq" / "fasta"): the
-    caller's choice, by the first byte of the file's first non-empty line.
+    caller's choice, by the first byte of the file's first non-empty line.  With BAM / BAM_ORIGINAL_STRAND (or "bam" / "bam_original_strand")
+    chunks are decompressed BAM record bytes, the header skipped, and the batch is kmc_b200.reads.bam_records_to_batch's (original_strand
+    for BAM_ORIGINAL_STRAND); a final chunk that ends inside a record and a malformed record raise ERR_INVALID.
 
     A chunk is parsed up to its last record end unless it is final (then to its end, as if it ended in '\n'); `consumed` says where the
     next chunk must start.  A record longer than the chunk is an error: since the limit here is raw bytes per chunk, a FASTQ record of more
@@ -741,13 +745,18 @@ class FastxParser(_Handle):
     _prefix = "kmcb200_fastx"
 
     def __init__(self, fmt, device=0, max_chunk_bytes=1 << 26):
-        self.format = {"fastq": FASTQ, "fasta": FASTA}.get(fmt, fmt) if isinstance(fmt, str) else int(fmt)
+        self.format = {"fastq": FASTQ, "fasta": FASTA, "bam": BAM, "bam_original_strand": BAM_ORIGINAL_STRAND}.get(fmt, fmt) \
+            if isinstance(fmt, str) else int(fmt)
         self.max_chunk_bytes = max_chunk_bytes
         p = _FastxParams(device, self.format, max_chunk_bytes)
         self._open(C.byref(p))
 
     def kernel_launches(self):
         return int(self.lib.kmcb200_fastx_kernel_launches(self._h))
+
+    def last_records(self):
+        """kmcb200_fastx_last_records: the records the latest host-buffer call parsed (parse or any handle's _fastx entry point)."""
+        return int(self.lib.kmcb200_fastx_last_records(self._h))
 
     def parse(self, raw, is_final=True, limit=None, out=None):
         """kmcb200_fastx_parse: (batch, consumed).  `out` (uint8, default: bytes + 1 fresh bytes) receives the batch; a shorter one than the
@@ -761,7 +770,7 @@ class FastxParser(_Handle):
 
     def dev_parse(self, d_raw, nbytes, is_final, limit, d_seq, seq_capacity, d_result, stream=None):
         """kmcb200_dev_fastx_parse: device pointers (ints or tensors' data_ptr()); seq_capacity >= nbytes + 1; d_result receives 4 x uint64:
-        consumed, sequence bytes, records, error flag (a non-final chunk without a record end)."""
+        consumed, sequence bytes, records, error (1: a non-final chunk without a record end; BAM: 2 truncated, 3 malformed)."""
         self._check(self.lib.kmcb200_dev_fastx_parse(self._h, d_raw, nbytes, int(bool(is_final)), FASTX_NO_LIMIT if limit is None else int(limit),
                                                      d_seq, seq_capacity, d_result, stream))
 

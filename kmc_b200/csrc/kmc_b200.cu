@@ -15,6 +15,7 @@
 #include "leaf_hash_wide.cuh"
 #include "split.cuh"
 #include "fastx.cuh"
+#include "bam.cuh"
 #include "hc.cuh"
 #include "small_k.cuh"
 #include "estimate.cuh"

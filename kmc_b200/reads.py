@@ -49,6 +49,18 @@ totals are those of the same text uncompressed.  As in the reference, a gzip fil
 (stage 0's sample budget, the estimator's s); the sample itself and the parser's limit count text bytes.
 
     python -m kmc_b200.reads --gpu-parse -k31 reads.fq.gz out_prefix
+
+BAM input (`kmc -fbam`): a gzip file whose text starts with "BAM\\1" is BAM, whatever its name.  It must be BGZF throughout and end with
+the 28-byte BGZF EOF member (as in the reference, binary_reader.h:159-174).  The header (text and references) is skipped; every record
+whose FLAG has neither 0x100 (secondary) nor 0x800 (supplementary) is one read, its SEQ decoded to A, C, G, T and N for every other code
+(CSplitter::GetSeq, splitter.cpp:326-418).  With both_strands=False (`-b`) the records of FLAG 0x10 are reverse complemented back to their
+original strand, as the reference does; canonical counting uses SEQ as stored, which gives the same k-mers but other super-k-mer cuts.
+parse="host" walks the records serially and decodes in numpy (bam_to_batch); parse="gpu" inflates the members on the GPU, skips the header
+on the reader thread and walks and decodes the records on the GPU (kmc_b200.FastxParser with BAM / BAM_ORIGINAL_STRAND).  A BAM file counts
+0.7 times its bytes in the predicted input size; stage 0's sample counts record bytes.  The files are the reference's for records shorter
+than 524,296 bases (its read buffer, kmc.h:419).
+
+    python -m kmc_b200.reads --gpu-parse -k31 reads.bam out_prefix
 """
 import argparse
 import json
@@ -62,7 +74,7 @@ import zlib
 
 import numpy as np
 
-from . import DbWriter, FASTA, FASTQ, FastxParser, Gunzip, HistogramEstimator, KmcB200Error, ERR_INVALID, SignatureStats, SmallKCounter, \
+from . import BAM, BAM_ORIGINAL_STRAND, DbWriter, FASTA, FASTQ, FastxParser, Gunzip, HistogramEstimator, KmcB200Error, ERR_INVALID, SignatureStats, SmallKCounter, \
     Splitter, Stage2Context, Stage2Params, bgzf_scan, signature_map as _signature_map, stage2_bin_order
 
 _NL, _GT, _AT = 10, ord(">"), ord("@")
@@ -72,6 +84,10 @@ GZIP_MAGIC = b"\x1f\x8b"
 GZIP_SIZE_FACTOR = 3.2                                                  # binary_reader.h:378-386: a gzip file's predicted text size
 BGZF_MAX_TEXT = 1 << 16                                                 # text of one BGZF member, at most
 _ZLIB_READ = 1 << 18                                                    # compressed bytes per zlib step on the reader thread
+BAM_MAGIC = b"BAM\1"
+BAM_SIZE_FACTOR = 0.7                                                   # binary_reader.h:368-371: a BAM file's predicted size
+BGZF_EOF = bytes.fromhex("1f8b08040000000000ff0600424302001b0003000000000000000000")   # the SAM/BAM specification's empty last member
+_BAM_FIXED = 36                                                         # block_size and the 32 bytes of fixed fields
 
 
 def is_gzip(path):
@@ -80,10 +96,30 @@ def is_gzip(path):
         return f.read(2) == GZIP_MAGIC
 
 
+def is_bam(path):
+    """A gzip file whose text starts with the BAM magic "BAM\\1" (decided on content: the name does not matter)."""
+    with open(path, "rb") as f:
+        data = f.read(1 << 16)
+    if data[:2] != GZIP_MAGIC:
+        return False
+    try:
+        return zlib.decompressobj(31).decompress(data, len(BAM_MAGIC)) == BAM_MAGIC
+    except zlib.error:
+        return False
+
+
+def _input_size(path):
+    size = os.path.getsize(path)
+    if is_bam(path):
+        return int(BAM_SIZE_FACTOR * size)
+    return int(GZIP_SIZE_FACTOR * size) if is_gzip(path) else size
+
+
 def predicted_size(paths):
-    """The input size the reference plans with (CBinaryFilesReader, binary_reader.h:378-386): a plain file counts its bytes, a gzip file
-    (uint64)(3.2 * its bytes).  The reference tells gzip by the name's ".gz", this library by the file's first bytes."""
-    return sum(int(GZIP_SIZE_FACTOR * os.path.getsize(p)) if is_gzip(p) else os.path.getsize(p) for p in paths)
+    """The input size the reference plans with (CBinaryFilesReader, binary_reader.h:360-386): a plain file counts its bytes, a gzip file
+    (uint64)(3.2 * its bytes), a BAM file (uint64)(0.7 * its bytes).  The reference tells gzip by the name's ".gz" and BAM by -fbam, this
+    library both by the file's first bytes."""
+    return sum(_input_size(p) for p in paths)
 
 
 def _gzip_error(e):
@@ -150,6 +186,206 @@ def sequences_to_batch(data):
     return a[keep]
 
 
+def _bam_error(msg):
+    return KmcB200Error(ERR_INVALID, "BAM input: %s" % msg)
+
+
+def check_bgzf_members(data):
+    """A BAM file's members: every one BGZF (its BC subfield gives its length), the last one the EOF member."""
+    if not data.endswith(BGZF_EOF):
+        raise _bam_error("wrong EOF marker (the file does not end with the BGZF EOF member)")
+    pos = 0
+    while pos < len(data):
+        size = _bgzf_member_size(data, pos)
+        if size is None:
+            raise _bam_error("member at byte %d is not BGZF" % pos)
+        pos += size
+    if pos != len(data):
+        raise _bam_error("the last member is truncated")
+
+
+def _bgzf_member_size(data, pos):
+    """BSIZE + 1 of the BGZF member at data[pos:], or None when it is not one: the gzip header with FEXTRA alone and a BC subfield of
+    length 2 among its extra subfields (any others are skipped), the rule kmcb200_bgzf_scan applies."""
+    if len(data) - pos < 12 or data[pos:pos + 4] != b"\x1f\x8b\x08\x04":
+        return None
+    xlen, = struct.unpack_from("<H", data, pos + 10)
+    end = pos + 12 + xlen
+    if end > len(data):
+        return None
+    q = pos + 12
+    while q + 4 <= end:
+        slen, = struct.unpack_from("<H", data, q + 2)
+        if data[q:q + 2] == b"BC" and slen == 2 and q + 6 <= end:
+            size = struct.unpack_from("<H", data, q + 4)[0] + 1
+            return size if size >= 12 + xlen + 8 + 2 else None
+        q += 4 + slen
+    return None
+
+
+class BamHeader:
+    """The BAM header (magic, l_text, text, n_ref, and l_name, name, l_ref of every reference), skipped piece by piece: feed(piece) returns
+    where the records start in the piece, or None while the whole piece is header.  A header may span any number of pieces."""
+
+    def __init__(self):
+        self.need, self.field, self.buf = 4, "magic", b""              # bytes still wanted for the current field
+        self.n_ref = 0
+        self.done = False
+
+    def feed(self, piece):
+        mv = memoryview(piece).cast("B")
+        pos = 0
+        while not self.done:
+            take = min(self.need, len(mv) - pos)
+            if self.field in ("text", "name"):                          # skipped bytes
+                self.need -= take
+            else:
+                self.buf += bytes(mv[pos:pos + take])
+                self.need -= take
+            pos += take
+            if self.need:
+                return None
+            self._next()
+        return pos
+
+    def _next(self):
+        f, v = self.field, self.buf
+        self.buf = b""
+        if f == "magic":
+            if v != BAM_MAGIC:
+                raise _bam_error("the text does not start with the BAM magic")
+            self.field, self.need = "l_text", 4
+        elif f == "l_text":
+            self.field, self.need = "text", self._count(v, "l_text")
+        elif f == "text":
+            self.field, self.need = "n_ref", 4
+        elif f == "n_ref":
+            self.n_ref = self._count(v, "n_ref")
+            self._ref_or_done()
+        elif f == "l_name":
+            self.field, self.need = "name", self._count(v, "l_name")
+        elif f == "name":
+            self.field, self.need = "l_ref", 4
+        else:                                                           # l_ref
+            self.n_ref -= 1
+            self._ref_or_done()
+        if self.field in ("text", "name") and self.need == 0:
+            self._next()
+
+    def _ref_or_done(self):
+        if self.n_ref:
+            self.field, self.need = "l_name", 4
+        else:
+            self.done = True
+
+    @staticmethod
+    def _count(v, name):
+        n = struct.unpack("<i", v)[0]
+        if n < 0:
+            raise _bam_error("negative %s in the header" % name)
+        return n
+
+    def finish(self):
+        if not self.done:
+            raise _bam_error("the header is truncated")
+
+
+def bam_records(data):
+    """The record bytes of a whole decompressed BAM file: the text after its header."""
+    h = BamHeader()
+    at = h.feed(data)
+    h.finish()
+    return memoryview(data)[at:]
+
+
+def bam_walk(records):
+    """The records of decompressed BAM record bytes, serially (CSplitter::GetSeq): (start, l_seq, flag, seq offset) per record.  A
+    block_size below 32, a negative l_seq, fixed fields longer than block_size, or bytes after the last whole record raise ERR_INVALID."""
+    out = []
+    p, n = 0, len(records)
+    while p < n:
+        if n - p < 4:
+            raise _bam_error("the last record is truncated")
+        bs = struct.unpack_from("<i", records, p)[0]
+        if bs < 32:
+            raise _bam_error("a malformed record at byte %d: block_size %d" % (p, bs))
+        if n - p - 4 < bs:
+            raise _bam_error("the last record is truncated")
+        l_name, n_cigar, flag, l_seq = records[p + 12], *struct.unpack_from("<HHi", records, p + 16)
+        if l_seq < 0 or 32 + l_name + 4 * n_cigar + (l_seq + 1) // 2 + l_seq > bs:
+            raise _bam_error("a malformed record at byte %d" % p)
+        out.append((p, l_seq, flag, p + _BAM_FIXED + l_name + 4 * n_cigar))
+        p += 4 + bs
+    return out
+
+
+def bam_record_end(records, at):
+    """End (exclusive) of the BAM record of `records` that contains byte `at` (records of a whole walk)."""
+    ends = np.array([r[0] for r in bam_walk(records)[1:]] + [len(records)], dtype=np.int64)
+    return int(ends[np.searchsorted(ends, at, side="right")])
+
+
+_BAM_BASE = np.frombuffer(b"NACNGNNNTNNNNNNN", dtype=np.uint8)      # =ACMGRSVTWYHKDBN: A C G T at codes 1 2 4 8, N elsewhere
+_BAM_COMP = np.frombuffer(b"NTGNCNNNANNNNNNN", dtype=np.uint8)
+
+
+def bam_records_to_batch(records, original_strand=False):
+    """Decompressed BAM record bytes -> the batch CSplitter::GetSeq reads: every record without FLAG 0x100 / 0x800 becomes its SEQ
+    (A C G T, N for every other code) and one newline; with original_strand, the records of FLAG 0x10 reverse complemented."""
+    a = _as_array(records)
+    recs = [r for r in bam_walk(records) if not r[2] & 0x900]
+    if not recs:
+        return np.zeros(0, dtype=np.uint8)
+    r = np.array(recs, dtype=np.int64)
+    lens, flags, seq = r[:, 1], r[:, 2], r[:, 3]
+    rev = (flags & 0x10) != 0 if original_strand else np.zeros(len(r), dtype=bool)
+    out = np.full(int(lens.sum()) + len(r), _NL, dtype=np.uint8)
+    out_off = np.concatenate([[0], np.cumsum(lens + 1)[:-1]])
+    cum = np.cumsum(lens)
+    i = 0
+    while i < len(r):                                                   # about 2^22 bases per step, at least one record
+        j = max(i + 1, int(np.searchsorted(cum, cum[i] - lens[i] + (1 << 22), side="right")))
+        ln = lens[i:j]
+        rid = np.repeat(np.arange(j - i), ln)
+        within = np.arange(int(ln.sum()), dtype=np.int64) - np.repeat(np.concatenate([[0], np.cumsum(ln)[:-1]]), ln)
+        rv = rev[i:j][rid]
+        k = np.where(rv, ln[rid] - 1 - within, within)
+        byte = a[seq[i:j][rid] + k // 2]
+        nib = np.where(k & 1, byte & 15, byte >> 4)
+        out[out_off[i:j][rid] + within] = np.where(rv, _BAM_COMP[nib], _BAM_BASE[nib])
+        i = j
+    return out
+
+
+def bam_to_batch(data, original_strand=False):
+    """A whole decompressed BAM file -> its batch: the header skipped, then bam_records_to_batch."""
+    return bam_records_to_batch(bam_records(data), original_strand)
+
+
+def read_bam(path):
+    """The decompressed text of a BAM file (every member checked to be BGZF, the EOF member last), inflated with zlib."""
+    with open(path, "rb") as f:
+        data = f.read()
+    check_bgzf_members(data)
+    return b"".join(_zlib_members(data))
+
+
+def bam_n_reads(records):
+    """The reads a BAM file gives: its records without FLAG 0x100 / 0x800."""
+    return sum(1 for r in bam_walk(records) if not r[2] & 0x900)
+
+
+def _read_input(path):
+    """(data, bam): a BAM file's record bytes (header skipped), or the text of a FASTQ / FASTA file."""
+    if is_bam(path):
+        return bam_records(read_bam(path)), True
+    return read_text(path), False
+
+
+def _to_batch(data, bam, original_strand=False):
+    return bam_records_to_batch(data, original_strand) if bam else sequences_to_batch(data)
+
+
 def batches(seq, batch_bytes):
     """Cuts a batch between records into pieces of at most batch_bytes (a record longer than that is an error)."""
     seps = np.flatnonzero(seq == _NL)
@@ -211,7 +447,8 @@ class _RawChunks:
     in turn with the next chunk_bytes / 2 bytes of the file, so reading the next piece overlaps the work on the current chunk.  Iterating
     gives (chunk, is_final); the caller reports how much of each non-final chunk it parsed with .consumed(n), and the rest (an unfinished
     record) is copied in front of the next piece, so every chunk starts on a record.  close() (or leaving the `with`) ends the thread.
-    A gzip file gives its text the same way, chunk_bytes / 2 text bytes per piece (_GzText)."""
+    A gzip file gives its text the same way, chunk_bytes / 2 text bytes per piece (_GzText); a BAM file its record bytes, the header
+    skipped on the reader thread (.bam is True)."""
 
     def __init__(self, path, chunk_bytes, device=0):
         self.size = os.path.getsize(path)
@@ -223,8 +460,15 @@ class _RawChunks:
             self.free.put(i)
         self.wait_s = 0.0                                               # time the consumer waited for the reader
         self._consumed = None
+        self.bam = is_bam(path)
         self._f = open(path, "rb")
-        self._gz = _GzText(self._f, self.piece, device) if is_gzip(path) else None
+        if self.bam:
+            self._f.seek(-min(len(BGZF_EOF), self.size), os.SEEK_END)
+            if self._f.read(len(BGZF_EOF)) != BGZF_EOF:
+                self._f.close()
+                raise _bam_error("wrong EOF marker (the file does not end with the BGZF EOF member)")
+            self._f.seek(0)
+        self._gz = _GzText(self._f, self.piece, device, bgzf_only=self.bam) if is_gzip(path) else None
         self._thread = threading.Thread(target=self._read if self._gz is None else self._read_gzip, name="kmc_b200-reader", daemon=True)
         self._thread.start()
 
@@ -245,12 +489,25 @@ class _RawChunks:
             self.full.put(e)
 
     def _read_gzip(self):
+        hdr = BamHeader() if self.bam else None                          # a BAM file's pieces hold record bytes only
         try:
             while True:
                 i = self.free.get()
                 if i is None:
                     return
-                n, final = self._gz.fill(self.bufs[i][1][self.head:self.head + self.piece])
+                out = self.bufs[i][1][self.head:self.head + self.piece]
+                while True:
+                    n, final = self._gz.fill(out)
+                    if hdr is not None and not hdr.done:
+                        at = hdr.feed(out[:n])
+                        if at is None:
+                            if final:
+                                hdr.finish()
+                            continue
+                        out[:n - at] = out[at:n].copy()
+                        n -= at
+                    if n or final:
+                        break
                 self.full.put((i, n, final))
                 if final:
                     return
@@ -312,10 +569,11 @@ class _GzText:
     """The text of a gzip file, piece by piece, for _RawChunks' reader thread.  BGZF members are inflated on the GPU (Gunzip, on its own
     stream, so this overlaps the parse and split of the previous chunk): compressed bytes are read into a pinned buffer, the whole members
     that fit the piece are inflated straight into it, and a partial member stays for the next read.  From the first member that is not BGZF
-    on (plain `gzip`, concatenated members, or a later part of a mixed file), zlib inflates the rest of the file, member after member."""
+    on (plain `gzip`, concatenated members, or a later part of a mixed file), zlib inflates the rest of the file, member after member;
+    with bgzf_only (BAM) such a member is an error."""
 
-    def __init__(self, f, piece, device):
-        self.f, self.piece, self.device = f, piece, device
+    def __init__(self, f, piece, device, bgzf_only=False):
+        self.f, self.piece, self.device, self.bgzf_only = f, piece, device, bgzf_only
         self.zcap = piece + (1 << 17)                                  # a piece of text in members, and the partial member after them
         self._zt, self.z = _pinned(self.zcap)
         self.zlen, self.eof = 0, False
@@ -344,6 +602,8 @@ class _GzText:
             if self.zlen == 0:
                 return n, True
             if not self._bgzf_next():
+                if self.bgzf_only:
+                    raise _bam_error("a member is not BGZF")
                 rest = bytes(self.z[:self.zlen])
                 self.zlen = 0
                 self.blocks = _zlib_members(rest, lambda: self.f.read(_ZLIB_READ))
@@ -386,8 +646,9 @@ class _Parsers:
     def __init__(self, device, max_chunk_bytes):
         self.device, self.max_chunk_bytes, self.by_format = device, max_chunk_bytes, {}
 
-    def __call__(self, chunk):
-        fmt = fastx_format(chunk)
+    def __call__(self, chunk, fmt=None):
+        """The parser of `fmt`, by default FASTQ or FASTA as the chunk's text says."""
+        fmt = fmt or fastx_format(chunk)
         if fmt not in self.by_format:
             self.by_format[fmt] = FastxParser(fmt, self.device, self.max_chunk_bytes)
         return self.by_format[fmt]
@@ -401,7 +662,8 @@ class _Parsers:
 def signature_sample_counts(paths, k, signature_len, batch_bytes=1 << 26, device=0, parse="host", homopolymer_compressed=False):
     """Stage 0's statistics (CKMC::buildSignatureMapping, kmc_core/kmc.h:974-1075): k-mers per signature, counted on the GPU, over the
     text of the files in input order up to the end of the first record at or beyond max(2^28, predicted_size / 100) text bytes (a gzip
-    file counts 3.2 times its bytes in the prediction, its text in the sample).
+    file counts 3.2 times its bytes in the prediction, its text in the sample; a BAM file 0.7 times its bytes, its record bytes).  BAM
+    records are counted as stored: a k-mer's signature is the same on either strand, so -b's reverse complement changes no count.
     parse="gpu": the files are parsed on the GPU in chunks of batch_bytes - 1, the sample's end found by the parser's limit.
     homopolymer_compressed: the k-mers of the compressed reads are counted (`kmc -hc`); the sample's end is still found on the raw bytes."""
     budget = max(STATS_SAMPLE_BYTES, predicted_size(paths) // 100)
@@ -416,7 +678,7 @@ def signature_sample_counts(paths, k, signature_len, batch_bytes=1 << 26, device
                 with _RawChunks(path, batch_bytes - 1, device) as chunks:
                     parser = None
                     for chunk, final in chunks:
-                        parser = parser or parsers(chunk)
+                        parser = parser or parsers(chunk, BAM if chunks.bam else None)
                         limit = budget - pos if cut else None
                         used = st.add_fastx(parser, chunk, final, limit)
                         chunks.consumed(used)
@@ -432,13 +694,13 @@ def signature_sample_counts(paths, k, signature_len, batch_bytes=1 << 26, device
     for path in paths:
         if budget <= 0:
             break
-        data = read_text(path)
-        if not data:
+        data, bam = _read_input(path)
+        if not len(data):
             continue
         if len(data) > budget:
-            data = data[:_record_end(data, budget - 1)]
+            data = data[:(bam_record_end if bam else _record_end)(data, budget - 1)]
         budget -= len(data)
-        for batch in batches(sequences_to_batch(data), batch_bytes):
+        for batch in batches(_to_batch(data, bam), batch_bytes):
             st.add(batch)
     counts = st.read()
     st.close()
@@ -452,7 +714,7 @@ ESTIMATE_LARGE_INPUT = 50_000_000_000                                   # kmc.h:
 
 def estimate_s(paths):
     """The reference's sampling exponent for these inputs: 7, or 11 when their predicted size (predicted_size: gzip files count 3.2 times
-    their bytes) is at least 5 * 10^10 bytes."""
+    their bytes, BAM files 0.7 times) is at least 5 * 10^10 bytes."""
     return 11 if predicted_size(paths) >= ESTIMATE_LARGE_INPUT else 7
 
 
@@ -507,13 +769,13 @@ def estimate_histogram(paths, k, s=None, batch_bytes=1 << 26, device=0, parse="h
                 with _RawChunks(path, batch_bytes - 1, device) as chunks:
                     parser = None
                     for chunk, final in chunks:
-                        parser = parser or parsers(chunk)
+                        parser = parser or parsers(chunk, BAM if chunks.bam else None)   # canonical hashes: either strand
                         chunks.consumed(est.add_fastx(parser, chunk, final))
                 continue
-            data = read_text(path)
-            if not data:
+            data, bam = _read_input(path)
+            if not len(data):
                 continue
-            for batch in batches(sequences_to_batch(data), batch_bytes):
+            for batch in batches(_to_batch(data, bam), batch_bytes):
                 est.add(batch)
         return est.histogram()
     finally:
@@ -550,15 +812,15 @@ def count_reads_small_k(paths, out_prefix, k, cutoff_min=2, cutoff_max=1_000_000
                 with _RawChunks(path, batch_bytes - 1, device) as chunks:
                     parser = None
                     for chunk, final in chunks:
-                        parser = parser or parsers(chunk)
+                        parser = parser or parsers(chunk, (BAM if both_strands else BAM_ORIGINAL_STRAND) if chunks.bam else None)
                         chunks.consumed(sk.add_fastx(parser, chunk, final))
                         n_bases += sk.last_seq_bytes
                 read_s += chunks.wait_s
                 continue
             t = time.perf_counter()
-            data = read_text(path)
+            data, bam = _read_input(path)
             read_s += time.perf_counter() - t
-            seq = sequences_to_batch(data)
+            seq = _to_batch(data, bam, not both_strands)
             del data
             for batch in batches(seq, batch_bytes):
                 sk.add(batch)
@@ -643,11 +905,13 @@ def count_reads(paths, out_prefix, k, signature_len, signature_map, lut_prefix_l
                 with _RawChunks(path, batch_bytes - 1, device) as chunks:
                     parser = None
                     for chunk, final in chunks:
-                        parser = parser or parsers(chunk)
+                        parser = parser or parsers(chunk, (BAM if both_strands else BAM_ORIGINAL_STRAND) if chunks.bam else None)
                         out, packs, frags, used, nseq = sp.split_fastx(parser, chunk, final)
                         if est is not None:
                             est.add_fastx(parser, chunk[:used], True)
                             n_reads += est.last_records
+                        elif chunks.bam:
+                            n_reads += parser.last_records()
                         else:
                             n_reads += n_records(chunk[:used])
                         chunks.consumed(used)
@@ -656,10 +920,10 @@ def count_reads(paths, out_prefix, k, signature_len, signature_map, lut_prefix_l
                 read_s += chunks.wait_s
                 continue
             t = time.perf_counter()
-            data = read_text(path)
+            data, bam = _read_input(path)
             read_s += time.perf_counter() - t
-            n_reads += n_records(data)
-            seq = sequences_to_batch(data)
+            n_reads += bam_n_reads(data) if bam else n_records(data)
+            seq = _to_batch(data, bam, not both_strands)
             del data
             for batch in batches(seq, batch_bytes):
                 out, packs, frags = sp.split_raw(batch)
@@ -715,7 +979,7 @@ def count_reads(paths, out_prefix, k, signature_len, signature_map, lut_prefix_l
 
 def main(argv=None):
     ap = argparse.ArgumentParser(prog="python -m kmc_b200.reads", description=__doc__.split("\n\n")[0])
-    ap.add_argument("inputs", nargs="+", help="FASTQ / FASTA files, then the output prefix")
+    ap.add_argument("inputs", nargs="+", help="FASTQ / FASTA / BAM files, then the output prefix")
     ap.add_argument("-k", type=int, default=25)
     ap.add_argument("-p", "--signature-len", type=int, default=9)
     ap.add_argument("-n", "--n-bins", type=int, default=None, help="bins when the map is chosen from the reads (default %d, KMC's -n)" % DEFAULT_N_BINS)

@@ -501,6 +501,58 @@ int kmcb200_gunzip_inflate(kmcb200_gunzip* p, const uint8_t* raw, uint64_t bytes
 int kmcb200_dev_gunzip_inflate(kmcb200_gunzip* p, const kmcb200_bgzf_member* d_members, uint64_t n_members, const uint8_t* d_raw, uint64_t raw_bytes,
 	uint8_t* d_text, uint64_t text_capacity, uint64_t* d_error, void* stream);
 
+/* ---- KMC database input (`kmc -fkmc`): .kmc_suf records decoded on the GPU into k-mer reads ----------------------------------------
+ * What the reference reads from a KMC database (CBinaryFilesReader::ProcessKMC through CKMCFile::ReadNextKmer, kmc_api/kmc_file.cpp:427-499):
+ * every record whose counter passes the database's cutoffs becomes one read, its k-mer.  A chunk is n_records whole records of .kmc_suf
+ * (after the "KMCS" marker), (k - lut_prefix_len) / 4 suffix bytes, most significant symbol first, then counter_size bytes, little-endian;
+ * first_record is the index of its first record in the file.  The batch is, per kept record in file order, its k symbols in ACGT and one
+ * '\n': the batch format of the splitter, the small-k counter and the estimator.
+ *   prefix    record g's lut_prefix_len leading symbols are #{ j >= 1 : lut[j] <= g } & (4^lut_prefix_len - 1) (the reference's listing
+ *             reader, CPrefixFileBufferForListingMode::GetPrefix).  `lut` is the LUT as that reader sees it: for a KMC2 database all its
+ *             n_bins * 4^lut_prefix_len + 1 stored words, for a KMC1 database its 4^lut_prefix_len stored words followed by total_kmers
+ *             (kmc_file.h:57-58).  It stays in HBM for the handle's lifetime and must be non-decreasing.
+ *   filter    counter_size 0: every record is kept.  Otherwise the counter, accumulated into a uint32, must lie in [min_count, max_count]
+ *             (the header's cutoffs; for KMC1 max_count is the 64-bit value of the header's two words).
+ * Work per call: 5 kernel launches whatever the size (count, a 3-launch scan, decode), no host synchronisation inside the device form.
+ * Workspace: the LUT, plus max_records * (record bytes + k + 1) bytes for the host-buffer form's chunk and output. */
+typedef struct kmcb200_kmcdb kmcb200_kmcdb;
+typedef struct {
+	int32_t device;                       /* CUDA ordinal */
+	uint32_t kmer_len;                    /* the database's k, 1..256 */
+	uint32_t lut_prefix_len;              /* 0..16, at most k, with (k - lut_prefix_len) % 4 == 0 */
+	uint32_t counter_size;                /* 0..4 (5..8 is KMCB200_ERR_INVALID: the reference's uint32 accumulation is undefined there) */
+	uint64_t min_count, max_count;        /* the header's cutoffs */
+	uint64_t total_kmers;                 /* records in .kmc_suf */
+	uint64_t max_records;                 /* largest chunk one call takes (1..KMCB200_SPLIT_MAX_BATCH / (k + 1)): sizes the workspace */
+} kmcb200_kmcdb_params;
+/* lut[0, lut_entries) as described above is copied to HBM.  KMCB200_ERR_INVALID for a bad parameter, KMCB200_ERR_NO_DEVICE without an
+ * sm_90 device (no CPU fallback). */
+int kmcb200_kmcdb_create(const kmcb200_kmcdb_params* params, const uint64_t* lut, uint64_t lut_entries, kmcb200_kmcdb** out);
+void kmcb200_kmcdb_destroy(kmcb200_kmcdb* d);
+const char* kmcb200_kmcdb_last_error(const kmcb200_kmcdb* d);
+/* Number of kernels this decoder has launched so far (the _kmcdb entry points below count theirs here too). */
+uint64_t kmcb200_kmcdb_kernel_launches(const kmcb200_kmcdb* d);
+/* Host buffers: copies the records in, returns when seq[0, *seq_bytes) holds the batch and *kept (optional) the records kept.  n_records
+ * above max_records or first_record + n_records above total_kmers: KMCB200_ERR_INVALID.  A batch longer than capacity:
+ * KMCB200_ERR_CAPACITY, *seq_bytes / *kept are set and seq is not written. */
+int kmcb200_kmcdb_decode(kmcb200_kmcdb* d, const uint8_t* suffix, uint64_t n_records, uint64_t first_record, uint8_t* seq, uint64_t capacity,
+	uint64_t* seq_bytes, uint64_t* kept);
+/* Device twin: d_suffix / d_seq / d_result in HBM, queued on `stream` (a cudaStream_t; NULL = the legacy default stream).  d_result receives
+ * 2 x uint64: [0] sequence bytes, [1] kept records; when [0] exceeds capacity d_seq is not written. */
+int kmcb200_dev_kmcdb_decode(kmcb200_kmcdb* d, const uint8_t* d_suffix, uint64_t n_records, uint64_t first_record, uint8_t* d_seq,
+	uint64_t capacity, uint64_t* d_result, void* stream);
+/* The records decoded straight into the handle's batch buffer, then what kmcb200_split / kmcb200_smallk_add / kmcb200_estimator_add do with
+ * a batch (homopolymer compression included, when it is on).  KMCB200_ERR_INVALID when n_records * (k + 1) exceeds the handle's
+ * max_batch_bytes, or for the chunk checks of kmcb200_kmcdb_decode.  *seq_bytes and *kept (optional) receive the batch's length and the
+ * records kept.  There is no signature-statistics form: the reference takes the signature map from the first input database. */
+int kmcb200_split_kmcdb(kmcb200_splitter* sp, kmcb200_kmcdb* d, const uint8_t* suffix, uint64_t n_records, uint64_t first_record,
+	uint8_t* out, uint64_t out_capacity, uint64_t* out_bytes, uint64_t* pack_bytes, uint64_t pack_capacity, uint64_t* n_packs,
+	kmcb200_bin_fragment* frags, uint64_t* seq_bytes, uint64_t* kept);
+int kmcb200_smallk_add_kmcdb(kmcb200_smallk* h, kmcb200_kmcdb* d, const uint8_t* suffix, uint64_t n_records, uint64_t first_record,
+	uint64_t* seq_bytes, uint64_t* kept);
+int kmcb200_estimator_add_kmcdb(kmcb200_estimator* h, kmcb200_kmcdb* d, const uint8_t* suffix, uint64_t n_records, uint64_t first_record,
+	uint64_t* seq_bytes, uint64_t* kept);
+
 /* ---- seam #1: sort host records ------------------------------------------------------------------
  * Contract of SortFunction (raduls.h:19-20, kb_sorter.h:775-779): n records of rec_bytes (multiple of 8,
  * CKmer<SIZE> images) sorted ascending on bytes key_bytes-1..0; the result is left in `tmp` when key_bytes

@@ -55,6 +55,11 @@ class _FastxParams(C.Structure):
     _fields_ = [("device", C.c_int32), ("format", C.c_uint32), ("max_chunk_bytes", C.c_uint64)]
 
 
+class _KmcDbParams(C.Structure):
+    _fields_ = [("device", C.c_int32), ("kmer_len", C.c_uint32), ("lut_prefix_len", C.c_uint32), ("counter_size", C.c_uint32),
+                ("min_count", C.c_uint64), ("max_count", C.c_uint64), ("total_kmers", C.c_uint64), ("max_records", C.c_uint64)]
+
+
 class _GunzipParams(C.Structure):
     _fields_ = [("device", C.c_int32), ("reserved", C.c_uint32), ("max_in_bytes", C.c_uint64), ("max_out_bytes", C.c_uint64)]
 
@@ -91,6 +96,8 @@ EXPORTS = [
     "kmcb200_estimator_histogram", "kmcb200_estimator_reset",
     "kmcb200_bgzf_scan", "kmcb200_gunzip_create", "kmcb200_gunzip_destroy", "kmcb200_gunzip_last_error", "kmcb200_gunzip_kernel_launches",
     "kmcb200_gunzip_inflate", "kmcb200_dev_gunzip_inflate",
+    "kmcb200_kmcdb_create", "kmcb200_kmcdb_destroy", "kmcb200_kmcdb_last_error", "kmcb200_kmcdb_kernel_launches", "kmcb200_kmcdb_decode",
+    "kmcb200_dev_kmcdb_decode", "kmcb200_split_kmcdb", "kmcb200_smallk_add_kmcdb", "kmcb200_estimator_add_kmcdb",
 ]
 
 FASTQ, FASTA, BAM, BAM_ORIGINAL_STRAND = 1, 2, 4, 5                    # KMCB200_FASTQ / _FASTA / _BAM / _BAM_ORIGINAL_STRAND
@@ -225,6 +232,18 @@ def load_library(build_if_needed=True):
     L.kmcb200_gunzip_kernel_launches.restype = u64
     L.kmcb200_gunzip_inflate.argtypes = [vp, vp, u64, vp, u64, C.POINTER(u64), C.POINTER(u64)]
     L.kmcb200_dev_gunzip_inflate.argtypes = [vp, vp, u64, vp, u64, vp, u64, vp, vp]
+    L.kmcb200_kmcdb_create.argtypes = [C.POINTER(_KmcDbParams), vp, u64, C.POINTER(vp)]
+    L.kmcb200_kmcdb_destroy.argtypes = [vp]
+    L.kmcb200_kmcdb_destroy.restype = None
+    L.kmcb200_kmcdb_last_error.argtypes = [vp]
+    L.kmcb200_kmcdb_last_error.restype = C.c_char_p
+    L.kmcb200_kmcdb_kernel_launches.argtypes = [vp]
+    L.kmcb200_kmcdb_kernel_launches.restype = u64
+    L.kmcb200_kmcdb_decode.argtypes = [vp, vp, u64, u64, vp, u64, C.POINTER(u64), C.POINTER(u64)]
+    L.kmcb200_dev_kmcdb_decode.argtypes = [vp, vp, u64, u64, vp, u64, vp, vp]
+    L.kmcb200_split_kmcdb.argtypes = [vp, vp, vp, u64, u64, vp, u64, C.POINTER(u64), vp, u64, C.POINTER(u64), vp, C.POINTER(u64), C.POINTER(u64)]
+    L.kmcb200_smallk_add_kmcdb.argtypes = [vp, vp, vp, u64, u64, C.POINTER(u64), C.POINTER(u64)]
+    L.kmcb200_estimator_add_kmcdb.argtypes = [vp, vp, vp, u64, u64, C.POINTER(u64), C.POINTER(u64)]
     _lib = L
     return L
 
@@ -534,6 +553,27 @@ class Splitter(_Handle):
             return self._out[:nbytes.value], self._packs[:npacks.value], list(frags), int(consumed.value), int(seq_bytes.value)
         raise KmcB200Error(ERR_CAPACITY, "kmcb200_split_fastx: buffers still too small")
 
+    def split_kmcdb(self, decoder, suffix, first_record):
+        """kmcb200_split_kmcdb: whole .kmc_suf records (bytes or a uint8 array, ideally pinned; first_record the index of the first) decoded
+        on the GPU by `decoder` (a KmcDbDecoder) straight into this splitter's batch buffer, then split like split_raw.  Returns
+        (out[:bytes], pack_bytes[:n_packs], fragments, seq_bytes, kept)."""
+        a = _as_u8(suffix)
+        n = decoder.records_in(a)
+        frags = (BinFragment * self.n_bins)()
+        nbytes, npacks, seq_bytes, kept = C.c_uint64(0), C.c_uint64(0), C.c_uint64(0), C.c_uint64(0)
+        for _ in range(2):
+            rc = self.lib.kmcb200_split_kmcdb(self._h, decoder._h, a.ctypes.data, n, int(first_record), self._out.ctypes.data, self._out.size,
+                                              C.byref(nbytes), self._packs.ctypes.data, self._packs.size, C.byref(npacks), frags,
+                                              C.byref(seq_bytes), C.byref(kept))
+            if rc == ERR_CAPACITY:
+                self._out = np.empty(int(nbytes.value * 1.25) + 1024, dtype=np.uint8)
+                self._packs = np.empty(int(npacks.value * 1.25) + 64, dtype=np.uint64)
+                continue
+            self._check(rc)
+            decoder.last_kept = int(kept.value)
+            return self._out[:nbytes.value], self._packs[:npacks.value], list(frags), int(seq_bytes.value), int(kept.value)
+        raise KmcB200Error(ERR_CAPACITY, "kmcb200_split_kmcdb: buffers still too small")
+
     def count_kxmers(self, both_strands=True):
         """From now on every split also counts, per bin, the collector's (k+x)-mers (n_plus_x_recs); zeroes the totals."""
         self._check(self.lib.kmcb200_splitter_count_kxmers(self._h, int(bool(both_strands))))
@@ -640,6 +680,17 @@ class SmallKCounter(_Handle):
         self.last_seq_bytes = int(seq_bytes.value)
         return int(consumed.value)
 
+    def add_kmcdb(self, decoder, suffix, first_record):
+        """kmcb200_smallk_add_kmcdb: whole .kmc_suf records decoded on the GPU by `decoder` (a KmcDbDecoder) and counted.  Returns the
+        records kept; the batch's length is left in last_seq_bytes."""
+        a = _as_u8(suffix)
+        seq_bytes, kept = C.c_uint64(0), C.c_uint64(0)
+        self._check(self.lib.kmcb200_smallk_add_kmcdb(self._h, decoder._h, a.ctypes.data, decoder.records_in(a), int(first_record),
+                                                      C.byref(seq_bytes), C.byref(kept)))
+        self.last_seq_bytes = decoder.last_seq_bytes = int(seq_bytes.value)
+        decoder.last_kept = int(kept.value)
+        return decoder.last_kept
+
     def read(self):
         """uint64[4^k]: the counts of every k-mer value so far."""
         out = np.zeros(1 << (2 * self.kmer_len), dtype=np.uint64)
@@ -710,6 +761,17 @@ class HistogramEstimator(_Handle):
         self.last_seq_bytes, self.last_records = int(seq_bytes.value), int(recs.value)
         return int(consumed.value)
 
+    def add_kmcdb(self, decoder, suffix, first_record):
+        """kmcb200_estimator_add_kmcdb: whole .kmc_suf records decoded on the GPU by `decoder` (a KmcDbDecoder) and hashed.  Returns the
+        records kept; the batch's length is left in last_seq_bytes."""
+        a = _as_u8(suffix)
+        seq_bytes, kept = C.c_uint64(0), C.c_uint64(0)
+        self._check(self.lib.kmcb200_estimator_add_kmcdb(self._h, decoder._h, a.ctypes.data, decoder.records_in(a), int(first_record),
+                                                         C.byref(seq_bytes), C.byref(kept)))
+        self.last_seq_bytes = decoder.last_seq_bytes = int(seq_bytes.value)
+        decoder.last_kept = int(kept.value)
+        return decoder.last_kept
+
     def read(self):
         """uint32[2, 2^27]: the two counter tables."""
         out = np.zeros((2, self.TABLE), dtype=np.uint32)
@@ -773,6 +835,49 @@ class FastxParser(_Handle):
         consumed, sequence bytes, records, error (1: a non-final chunk without a record end; BAM: 2 truncated, 3 malformed)."""
         self._check(self.lib.kmcb200_dev_fastx_parse(self._h, d_raw, nbytes, int(bool(is_final)), FASTX_NO_LIMIT if limit is None else int(limit),
                                                      d_seq, seq_capacity, d_result, stream))
+
+
+class KmcDbDecoder(_Handle):
+    """KMC database records -> batch on one GPU (kmcb200_kmcdb_*), what `kmc -fkmc` reads: every .kmc_suf record whose counter passes the
+    database's cutoffs becomes its k-mer in ACGT and one '\\n', in file order, byte for byte kmc_b200.reads.kmc_db_to_batch.  `lut` is the
+    LUT as the reference's listing reader sees it (kmc_b200.reads.kmc_db_info gives it); it stays in HBM.  A chunk is whole records, of
+    at most max_records; first_record is the index of its first record in the file."""
+    _prefix = "kmcb200_kmcdb"
+
+    def __init__(self, kmer_len, lut_prefix_len, counter_size, min_count, max_count, total_kmers, lut, device=0, max_records=1 << 22):
+        self.kmer_len, self.lut_prefix_len, self.counter_size = int(kmer_len), int(lut_prefix_len), int(counter_size)
+        self.record_bytes = (self.kmer_len - self.lut_prefix_len) // 4 + self.counter_size
+        self.max_records = int(max_records)
+        self.last_kept = self.last_seq_bytes = 0
+        lut = np.ascontiguousarray(lut, dtype=np.uint64)
+        p = _KmcDbParams(device, self.kmer_len, self.lut_prefix_len, self.counter_size, int(min_count), min(int(max_count), (1 << 64) - 1),
+                         int(total_kmers), self.max_records)
+        self._open(C.byref(p), lut.ctypes.data, lut.size)
+
+    def kernel_launches(self):
+        return int(self.lib.kmcb200_kmcdb_kernel_launches(self._h))
+
+    def records_in(self, a):
+        if self.record_bytes and a.size % self.record_bytes:
+            raise KmcB200Error(ERR_INVALID, "%d bytes are not whole records of %d bytes" % (a.size, self.record_bytes))
+        return a.size // self.record_bytes if self.record_bytes else 0
+
+    def decode(self, suffix, first_record, out=None):
+        """kmcb200_kmcdb_decode: the batch of the records (a uint8 view of `out`, default fresh n * (k + 1) bytes); a shorter `out` than
+        the batch raises ERR_CAPACITY and is left untouched.  The records kept are left in last_kept."""
+        a = _as_u8(suffix)
+        n = self.records_in(a)
+        o = np.empty(n * (self.kmer_len + 1), dtype=np.uint8) if out is None else out
+        nbytes, kept = C.c_uint64(0), C.c_uint64(0)
+        rc = self.lib.kmcb200_kmcdb_decode(self._h, a.ctypes.data, n, int(first_record), o.ctypes.data, o.size, C.byref(nbytes), C.byref(kept))
+        self.last_seq_bytes, self.last_kept = int(nbytes.value), int(kept.value)
+        self._check(rc)
+        return o[:nbytes.value]
+
+    def dev_decode(self, d_suffix, n_records, first_record, d_seq, capacity, d_result, stream=None):
+        """kmcb200_dev_kmcdb_decode: device pointers (ints or tensors' data_ptr()); d_result receives 2 x uint64: sequence bytes, records
+        kept (d_seq is not written when the first exceeds capacity)."""
+        self._check(self.lib.kmcb200_dev_kmcdb_decode(self._h, d_suffix, int(n_records), int(first_record), d_seq, int(capacity), d_result, stream))
 
 
 class Gunzip(_Handle):

@@ -16,6 +16,7 @@
 #include "split.cuh"
 #include "fastx.cuh"
 #include "bam.cuh"
+#include "kmcdb.cuh"
 #include "hc.cuh"
 #include "small_k.cuh"
 #include "estimate.cuh"
@@ -1704,4 +1705,5 @@ int kmcb200_leaf_plan(kmcb200_ctx* ctx, uint32_t slot, uint32_t* out)
 #include "fastx.inl"
 #include "small_k.inl"
 #include "estimate.inl"
+#include "kmcdb.inl"
 #include "gunzip.inl"

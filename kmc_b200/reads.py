@@ -61,6 +61,16 @@ on the reader thread and walks and decodes the records on the GPU (kmc_b200.Fast
 than 524,296 bases (its read buffer, kmc.h:419).
 
     python -m kmc_b200.reads --gpu-parse -k31 reads.bam out_prefix
+
+KMC database input (`kmc -fkmc`): an input named by its prefix, where P.kmc_pre and P.kmc_suf exist, is a KMC database; either every
+input is one or none is.  Every record whose counter passes the database's own cutoffs is one read, its k-mer (CKMCFile::ReadNextKmer,
+printed as FASTA by CBinaryFilesReader::ProcessKMC); a k above the database's gives no k-mers.  KMC1 and KMC2 databases are read; on the
+bin path stage 0 is skipped and the signature map is the first database's (kmc_input_signature_map: it must be KMC2, with the same
+signature length and number of bins, or the run is refused with the reference's message).  n_reads counts the kept records, and the
+predicted input size is the last database's total_kmers.  parse="host" decodes in numpy (kmc_db_to_batch); parse="gpu" reads .kmc_suf
+in chunks of whole records on a reader thread and decodes them on the GPU (kmc_b200.KmcDbDecoder).
+
+    python -m kmc_b200.reads --gpu-parse -k25 db31 out_prefix
 """
 import argparse
 import json
@@ -74,7 +84,7 @@ import zlib
 
 import numpy as np
 
-from . import BAM, BAM_ORIGINAL_STRAND, DbWriter, FASTA, FASTQ, FastxParser, Gunzip, HistogramEstimator, KmcB200Error, ERR_INVALID, SignatureStats, SmallKCounter, \
+from . import BAM, BAM_ORIGINAL_STRAND, DbWriter, FASTA, FASTQ, FastxParser, Gunzip, HistogramEstimator, KmcB200Error, KmcDbDecoder, ERR_INVALID, SignatureStats, SmallKCounter, \
     Splitter, Stage2Context, Stage2Params, bgzf_scan, signature_map as _signature_map, stage2_bin_order
 
 _NL, _GT, _AT = 10, ord(">"), ord("@")
@@ -118,7 +128,10 @@ def _input_size(path):
 def predicted_size(paths):
     """The input size the reference plans with (CBinaryFilesReader, binary_reader.h:360-386): a plain file counts its bytes, a gzip file
     (uint64)(3.2 * its bytes), a BAM file (uint64)(0.7 * its bytes).  The reference tells gzip by the name's ".gz" and BAM by -fbam, this
-    library both by the file's first bytes."""
+    library both by the file's first bytes.  KMC database input (every path a database prefix) is the last database's total_kmers: the
+    reference assigns it rather than adding it up (binary_reader.h:372-375)."""
+    if _kmc_inputs(paths):
+        return _kmc_predicted_size(paths)
     return sum(_input_size(p) for p in paths)
 
 
@@ -410,6 +423,238 @@ def signature_map_from_kmc_pre(path):
     sig_len = struct.unpack("<I", pre[h + 16:h + 20])[0]
     n = (1 << (2 * sig_len)) + 1
     return sig_len, np.frombuffer(pre[h - 4 * n:h], dtype=np.uint32).copy()
+
+
+KMC_PRE_MARKER, KMC_SUF_MARKER = b"KMCP", b"KMCS"
+KMC1_VERSION, KMC2_VERSION = 0, 0x200
+_KMC_ACGT = np.frombuffer(b"ACGT", dtype=np.uint8)
+_KMC_NOT_V2 = ("currently only KMC databases in version 2 can be readed. If needed to read other version please post an GitHub issue.")
+
+
+def is_kmc_db(path):
+    """`path` names a KMC database by its prefix: path.kmc_pre and path.kmc_suf both exist (what `kmc -fkmc` takes)."""
+    return os.path.isfile(path + ".kmc_pre") and os.path.isfile(path + ".kmc_suf")
+
+
+def _kmc_inputs(paths):
+    """True when every input is a KMC database, False when none is: kmc's -f applies to all inputs."""
+    db = [is_kmc_db(p) for p in paths]
+    if any(db) and not all(db):
+        raise KmcB200Error(ERR_INVALID, "either every input is a KMC database or none is (kmc's -f applies to all inputs)")
+    return bool(db) and all(db)
+
+
+class KmcDbInfo:
+    """The header of a KMC database as the reference's reader takes it (CKMCFile::ReadParamsFrom_prefix_file_buf, kmc_file.cpp:178-325),
+    and the LUT as its listing reader sees it: for KMC2 every stored word, for KMC1 the 4^lut_prefix_len stored words followed by
+    total_kmers (the guard of kmc_file.h:57-58).  n_bins and signature_map (the stored file positions) are those of a KMC2 database."""
+
+    def __init__(self, prefix):
+        self.prefix = prefix
+        with open(prefix + ".kmc_pre", "rb") as f:
+            pre = f.read()
+        if len(pre) < 16 or pre[:4] != KMC_PRE_MARKER or pre[-4:] != KMC_PRE_MARKER:
+            raise KmcB200Error(ERR_INVALID, "%s.kmc_pre is not a KMC database (no KMCP markers)" % prefix)
+        u32 = lambda at: struct.unpack_from("<I", pre, at)[0]                                            # noqa: E731
+        self.version = u32(len(pre) - 12)
+        if self.version not in (KMC1_VERSION, KMC2_VERSION):
+            raise KmcB200Error(ERR_INVALID, "%s.kmc_pre: version word %#x is neither KMC1 (0) nor KMC2 (0x200)" % (prefix, self.version))
+        header_offset = u32(len(pre) - 8)
+        h = len(pre) - 8 - header_offset
+        self.kmer_len, mode, self.counter_size, self.lut_prefix_len = (u32(h + 4 * i) for i in range(4))
+        if mode != 0:
+            raise KmcB200Error(ERR_INVALID, "%s: Quake compatible counters are not supported anymore" % prefix)
+        if self.counter_size > 4:
+            raise KmcB200Error(ERR_INVALID, "%s: counters of %d bytes are not read (the reference accumulates a counter into 32 bits)"
+                               % (prefix, self.counter_size))
+        if self.lut_prefix_len > self.kmer_len or (self.kmer_len - self.lut_prefix_len) % 4:
+            raise KmcB200Error(ERR_INVALID, "%s: lut_prefix_len %d does not fit k = %d" % (prefix, self.lut_prefix_len, self.kmer_len))
+        lut_words = 1 << (2 * self.lut_prefix_len)
+        if self.version == KMC2_VERSION:
+            self.signature_len, self.min_count, self.max_count = u32(h + 16), u32(h + 20), u32(h + 24)
+            self.total_kmers = struct.unpack_from("<Q", pre, h + 28)[0]
+            self.both_strands = pre[h + 36] == 0
+            map_size = (1 << (2 * self.signature_len)) + 1
+            map_at = h - 4 * map_size
+            self.lut = np.frombuffer(pre, dtype=np.uint64, count=(map_at - 4) // 8, offset=4).copy()
+            self.n_bins = (map_at - 4 - 8) // (8 * lut_words)
+            self.signature_map = np.frombuffer(pre, dtype=np.uint32, count=map_size, offset=map_at).copy()
+        else:
+            self.signature_len, self.min_count = None, u32(h + 16)
+            self.total_kmers = struct.unpack_from("<Q", pre, h + 24)[0]
+            self.both_strands = pre[h + 32] == 0
+            self.max_count = u32(h + 20) + (u32(h + 33) << 32)
+            self.lut = np.append(np.frombuffer(pre, dtype=np.uint64, count=lut_words, offset=4), np.uint64(self.total_kmers))
+            self.n_bins = self.signature_map = None
+        self.suffix_bytes = (self.kmer_len - self.lut_prefix_len) // 4
+        self.record_bytes = self.suffix_bytes + self.counter_size
+        suf_size = os.path.getsize(prefix + ".kmc_suf")
+        if suf_size < 4 + self.total_kmers * self.record_bytes:
+            raise KmcB200Error(ERR_INVALID, "%s.kmc_suf holds fewer than total_kmers = %d records" % (prefix, self.total_kmers))
+
+    def decoder(self, device=0, max_records=1 << 22):
+        """A KmcDbDecoder of this database with its LUT on the GPU."""
+        return KmcDbDecoder(self.kmer_len, self.lut_prefix_len, self.counter_size, self.min_count, self.max_count, self.total_kmers,
+                            self.lut, device, max_records)
+
+
+def kmc_db_info(prefix):
+    """The header and the listing LUT of the KMC database `prefix` (KmcDbInfo).  ERR_INVALID for what the reference refuses to read
+    (neither version 0 nor 0x200, Quake-compatible counters) and for counters of more than 4 bytes."""
+    return KmcDbInfo(prefix)
+
+
+def kmc_db_records(info):
+    """The records of .kmc_suf, uint8[total_kmers, record_bytes] (after the KMCS marker)."""
+    with open(info.prefix + ".kmc_suf", "rb") as f:
+        if f.read(4) != KMC_SUF_MARKER:
+            raise KmcB200Error(ERR_INVALID, "%s.kmc_suf does not start with KMCS" % info.prefix)
+        data = np.fromfile(f, dtype=np.uint8, count=info.total_kmers * info.record_bytes)
+    return data.reshape(info.total_kmers, info.record_bytes)
+
+
+def kmc_records_to_batch(info, recs, first_record):
+    """The host model of KmcDbDecoder: records first_record .. (uint8[n, record_bytes]) -> the batch, every kept record's k-mer in ACGT
+    and '\\n' (CKMCFile::ReadNextKmer, kmc_file.cpp:427-499, printed by CBinaryFilesReader::ProcessKMC, binary_reader.h:238-304)."""
+    recs = np.asarray(recs, dtype=np.uint8).reshape(-1, info.record_bytes)
+    g = np.arange(first_record, first_record + recs.shape[0], dtype=np.uint64)
+    if info.counter_size:
+        cnt = np.zeros(recs.shape[0], dtype=np.uint64)
+        for b in range(info.counter_size):
+            cnt |= recs[:, info.suffix_bytes + b].astype(np.uint64) << np.uint64(8 * b)
+        keep = (cnt >= info.min_count) & (cnt <= min(int(info.max_count), (1 << 64) - 1))
+        recs, g = recs[keep], g[keep]
+    k, lp = info.kmer_len, info.lut_prefix_len
+    prefix = np.searchsorted(info.lut[1:], g, side="right").astype(np.uint64) & np.uint64((1 << (2 * lp)) - 1)
+    out = np.empty((recs.shape[0], k + 1), dtype=np.uint8)
+    for i in range(lp):
+        out[:, i] = _KMC_ACGT[(prefix >> np.uint64(2 * (lp - 1 - i))) & np.uint64(3)]
+    for j in range(4):
+        out[:, lp + j:k:4] = _KMC_ACGT[(recs[:, :info.suffix_bytes] >> (6 - 2 * j)) & 3]
+    out[:, k] = _NL
+    return out.reshape(-1)
+
+
+def kmc_db_to_batch(prefix):
+    """The batch `kmc -fkmc` reads from the KMC database `prefix`: kmc_records_to_batch of all its records."""
+    info = kmc_db_info(prefix)
+    return kmc_records_to_batch(info, kmc_db_records(info), 0)
+
+
+def kmc_input_signature_map(prefix, signature_len, n_bins=None):
+    """CSignatureMapper::InitKMC (kmc_core/s_mapper.h:47-140): the signature map of a bin-path run on KMC database input, taken from the
+    first database.  The stored map values (file positions) are grouped in ascending order and the groups numbered 0, 1, ...; the special
+    signature 4^p goes to n_bins - 1 and its group does not advance the number.  Returns (int64[4^p + 1], n_bins).  n_bins=None takes
+    the database's number of LUT arrays; like kmc, ERR_INVALID for a KMC1 database, another signature length or another n_bins."""
+    info = kmc_db_info(prefix)
+    if info.version != KMC2_VERSION:
+        raise KmcB200Error(ERR_INVALID, _KMC_NOT_V2)
+    if info.signature_len != signature_len:
+        raise KmcB200Error(ERR_INVALID, "Wrong signature length, should be the same as input KMC database: %d" % info.signature_len)
+    if n_bins is not None and int(n_bins) != info.n_bins:
+        raise KmcB200Error(ERR_INVALID, "Wrong number of bins, should be the same as input KMC database: %d" % info.n_bins)
+    stored = info.signature_map
+    special = stored.size - 1
+    order = np.argsort(stored, kind="stable")
+    vals = stored[order]
+    group = np.cumsum(np.r_[True, vals[1:] != vals[:-1]]) - 1
+    special_group = group[np.flatnonzero(order == special)[0]]
+    bins = np.empty(stored.size, dtype=np.int64)
+    bins[order] = group - (group > special_group)
+    bins[special] = info.n_bins - 1
+    return bins, info.n_bins
+
+
+def _kmc_predicted_size(paths):
+    """binary_reader.h:372-375: with KMC input the predicted size is the last database's total_kmers (assigned, not added)."""
+    return kmc_db_info(paths[-1]).total_kmers if paths else 0
+
+
+class _KmcSufChunks:
+    """The records of one KMC database as chunks of at most max_records whole records in pinned host memory, read by a reader thread into
+    two buffers in turn, so reading the next chunk overlaps the work on the current one.  Iterating gives (records, first_record)."""
+
+    def __init__(self, info, max_records):
+        self.info, self.per = info, max(1, int(max_records))
+        nbytes = self.per * info.record_bytes
+        self.bufs = [_pinned(max(1, nbytes)) for _ in range(2)]
+        self.free, self.full = queue.Queue(), queue.Queue()
+        for i in range(2):
+            self.free.put(i)
+        self.wait_s = 0.0
+        self._f = open(info.prefix + ".kmc_suf", "rb")
+        if self._f.read(4) != KMC_SUF_MARKER:
+            self._f.close()
+            raise KmcB200Error(ERR_INVALID, "%s.kmc_suf does not start with KMCS" % info.prefix)
+        self._thread = threading.Thread(target=self._read, name="kmc_b200-kmc-reader", daemon=True)
+        self._thread.start()
+
+    def _read(self):
+        try:
+            first = 0
+            while first < self.info.total_kmers:
+                i = self.free.get()
+                if i is None:
+                    return
+                n = min(self.per, self.info.total_kmers - first)
+                want = n * self.info.record_bytes
+                if self._f.readinto(memoryview(self.bufs[i][1])[:want]) != want:
+                    raise KmcB200Error(ERR_INVALID, "short read: the file changed while it was read")
+                self.full.put((i, want, first))
+                first += n
+            self.full.put(None)
+        except BaseException as e:  # noqa: BLE001 - handed to the consumer
+            self.full.put(e)
+
+    def __iter__(self):
+        prev = None
+        while True:
+            t = time.perf_counter()
+            item = self.full.get()
+            self.wait_s += time.perf_counter() - t
+            if prev is not None:
+                self.free.put(prev)
+            if isinstance(item, BaseException):
+                raise item
+            if item is None:
+                return
+            i, want, first = item
+            prev = i
+            yield self.bufs[i][1][:want], first
+
+    def close(self):
+        if self._thread.is_alive():
+            self.free.put(None)
+            self.free.put(None)
+            self._thread.join()
+        self._f.close()
+
+    def __enter__(self):
+        return self
+
+    def __exit__(self, *exc):
+        self.close()
+
+
+def _kmc_chunks(paths, batch_bytes, device, parse):
+    """The databases' records in chunks whose batch fits batch_bytes: (info, decoder, records, first_record, batch) per chunk.
+    parse="host": decoder and records are None and batch is the numpy model's (kmc_records_to_batch).  parse="gpu": .kmc_suf is read on a
+    reader thread into pinned buffers, batch is None, and the caller decodes the records on the GPU with the decoder (KmcDbDecoder)."""
+    for path in paths:
+        info = kmc_db_info(path)
+        per = max(1, batch_bytes // (info.kmer_len + 1))
+        if parse == "gpu":
+            dec = info.decoder(device, per)
+            try:
+                with _KmcSufChunks(info, per) as chunks:
+                    for recs, first in chunks:
+                        yield info, dec, recs, first, None
+            finally:
+                dec.close()
+            continue
+        recs = kmc_db_records(info)
+        for first in range(0, info.total_kmers, per):
+            yield info, None, None, first, kmc_records_to_batch(info, recs[first:first + per], first)
 
 
 def _record_end(data, at):
@@ -762,6 +1007,16 @@ def estimate_histogram(paths, k, s=None, batch_bytes=1 << 26, device=0, parse="h
     if parse not in ("host", "gpu"):
         raise KmcB200Error(ERR_INVALID, "parse must be 'host' or 'gpu', not %r" % (parse,))
     est = HistogramEstimator(k, estimate_s(paths) if s is None else s, device, max_batch_bytes=batch_bytes)
+    if _kmc_inputs(paths):
+        try:
+            for _, dec, recs, first, batch in _kmc_chunks(paths, batch_bytes, device, parse):
+                if dec is None:
+                    est.add(batch)
+                else:
+                    est.add_kmcdb(dec, recs, first)
+            return est.histogram()
+        finally:
+            est.close()
     parsers = _Parsers(device, batch_bytes - 1) if parse == "gpu" else None
     try:
         for path in paths:
@@ -805,9 +1060,17 @@ def count_reads_small_k(paths, out_prefix, k, cutoff_min=2, cutoff_max=1_000_000
     sk = SmallKCounter(k, both_strands, device, max_batch_bytes=batch_bytes, homopolymer_compressed=homopolymer_compressed)
     n_bases = 0
     read_s = 0.0
-    parsers = _Parsers(device, batch_bytes - 1) if parse == "gpu" else None
+    kmc_input = _kmc_inputs(paths)
+    parsers = _Parsers(device, batch_bytes - 1) if parse == "gpu" and not kmc_input else None
     try:
-        for path in paths:
+        for _, dec, recs, first, batch in _kmc_chunks(paths, batch_bytes, device, parse) if kmc_input else ():
+            if dec is None:
+                sk.add(batch)
+                n_bases += batch.size
+            else:
+                sk.add_kmcdb(dec, recs, first)
+                n_bases += sk.last_seq_bytes
+        for path in paths if not kmc_input else ():
             if parsers is not None:
                 with _RawChunks(path, batch_bytes - 1, device) as chunks:
                     parser = None
@@ -871,7 +1134,13 @@ def count_reads(paths, out_prefix, k, signature_len, signature_map, lut_prefix_l
         return count_reads_small_k(paths, out_prefix, k, cutoff_min, cutoff_max, counter_max, both_strands, batch_bytes, device, parse,
                                    homopolymer_compressed)
     t0 = time.perf_counter()
-    if signature_map is None:
+    kmc_input = _kmc_inputs(paths)
+    if kmc_input:                                                       # stage 0 is skipped: the map comes from the first database
+        if signature_map is not None:
+            raise KmcB200Error(ERR_INVALID, "KMC database input takes its signature map from the first database: give signature_map=None")
+        mapper, n_bins = kmc_input_signature_map(paths[0], signature_len, n_bins)
+        sig_map = mapper.astype(np.uint32)
+    elif signature_map is None:
         n_bins = DEFAULT_N_BINS if n_bins is None else int(n_bins)
         mapper = _signature_map(signature_sample_counts(paths, k, signature_len, batch_bytes, device, parse, homopolymer_compressed),
                                 signature_len, n_bins)
@@ -898,9 +1167,22 @@ def count_reads(paths, out_prefix, k, signature_len, signature_map, lut_prefix_l
                 n_super += int(fr.n_super_kmers)
                 n_kmers += int(fr.n_rec)
 
-    parsers = _Parsers(device, batch_bytes - 1) if parse == "gpu" else None
+    parsers = _Parsers(device, batch_bytes - 1) if parse == "gpu" and not kmc_input else None
     try:
-        for path in paths:
+        for info, dec, recs, first, batch in _kmc_chunks(paths, batch_bytes, device, parse) if kmc_input else ():
+            if dec is None:
+                out, packs, frags = sp.split_raw(batch)
+                nseq, kept = batch.size, batch.size // (info.kmer_len + 1)
+                if est is not None:
+                    est.add(batch)
+            else:
+                out, packs, frags, nseq, kept = sp.split_kmcdb(dec, recs, first)
+                if est is not None:
+                    est.add_kmcdb(dec, recs, first)
+            n_reads += kept
+            n_bases += nseq
+            keep(out, packs, frags)
+        for path in paths if not kmc_input else ():
             if parsers is not None:
                 with _RawChunks(path, batch_bytes - 1, device) as chunks:
                     parser = None
@@ -979,7 +1261,7 @@ def count_reads(paths, out_prefix, k, signature_len, signature_map, lut_prefix_l
 
 def main(argv=None):
     ap = argparse.ArgumentParser(prog="python -m kmc_b200.reads", description=__doc__.split("\n\n")[0])
-    ap.add_argument("inputs", nargs="+", help="FASTQ / FASTA / BAM files, then the output prefix")
+    ap.add_argument("inputs", nargs="+", help="FASTQ / FASTA / BAM files or KMC database prefixes, then the output prefix")
     ap.add_argument("-k", type=int, default=25)
     ap.add_argument("-p", "--signature-len", type=int, default=9)
     ap.add_argument("-n", "--n-bins", type=int, default=None, help="bins when the map is chosen from the reads (default %d, KMC's -n)" % DEFAULT_N_BINS)
@@ -1024,7 +1306,7 @@ def main(argv=None):
         print(json.dumps(count_reads_small_k(a.inputs[:-1], a.inputs[-1], a.k, a.ci, a.cx, a.cs, not a.b, a.batch_bytes, a.device, parse, a.hc)))
         return 0
     lp = a.lut_prefix_len
-    if lp is None and not a.opt_out_size:
+    if lp is None and not a.opt_out_size and not _kmc_inputs(a.inputs[:-1]):     # KMC input: kmc's rule (from 4 * n_reads)
         lp = next(p for p in (7, 3, 11, 15, 4, 5, 6, 2, 8, 9, 10, 12, 13, 14, 1) if p < a.k and (a.k - p) % 4 == 0)
     res = count_reads(a.inputs[:-1], a.inputs[-1], a.k, m, sig_map, lp, a.ci, a.cx, a.cs, not a.b, a.batch_bytes, a.device,
                       a.n_bins if sig_map is None else None, parse=parse, small_k=False, opt_out_size=a.opt_out_size, homopolymer_compressed=a.hc)
